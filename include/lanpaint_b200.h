@@ -142,8 +142,7 @@ int lp_last_cuda_error(void); /* cudaError_t of the last failed launch on this t
  *   "tma" 1|0      use the TMA-staged persistent variants (cp.async.bulk + mbarrier ring) of the fused sub-step
  *                  (philox and torch streams) and of the step-boundary kernel when eligible: spatial a multiple
  *                  of 16, no side outputs, no row split (default 1; 2..5 select alternative tile geometries of
- *                  the philox kernel and 8 the two-subsequences-per-thread geometry of the torch kernel, for
- *                  measurement)
+ *                  the philox kernel, for measurement)
  *   "tma_min"      smallest launch, in elements, that takes a TMA-staged variant (default 2^18)
  *   "tma_boundary" 1|0  lp_boundary: TMA-staged kernel when eligible | always the LDG kernel (default 0: measured
  *                  faster inside a job, where the network's output is still in L2) */
@@ -188,6 +187,31 @@ int lp_torch_randn_geometry(int64_t numel, int device, int64_t* grid_out, uint64
 /* mask_f32 > 0.5 -> uint8 (the binarise of nodes.py:281-283, done once). */
 int lp_pack_mask_f32(const float* mask_f32, uint8_t* mask_u8, int64_t n, int invert, lp_stream_t stream);
 
+/* The known-operand layout.  The clean latent y and the noise image are only ever read at known positions
+ * (lanpaint.py:85-94,151-154,182-184), and both are constant for a whole job, so the kernels that stream them
+ * can read them packed: only their known elements, in element order.  Over the flat element index i of the
+ * latent (total = n_rows * per_row elements), with W = ceil(total / 32):
+ *   words[2w]     known bits of elements 32w .. 32w+31 (bit b <-> element 32w + b; 0 past the end)
+ *   words[2w + 1] number of known elements before element 32w, i.e. the packed index of the first known one
+ *   words[2W], words[2W + 1] = 0, number of known elements (end sentinel)
+ * so a known element i sits at packed index words[2w+1] + popc(words[2w] & ((1 << (i & 31)) - 1)), w = i >> 5.
+ * The bits follow the uint8 mask through its strides, so a channel-broadcast mask and a full-shape one give the
+ * same layout.  words holds lp_known_words(total) uint32 (the tail is the builder's scratch); y_known and
+ * noise_known hold total + 4 floats (the TMA-staged kernels fetch 16-byte aligned spans that may reach 3 floats
+ * past the last known element). */
+typedef struct lp_known {
+  const uint32_t* words;
+  const float* y;     /* y at known elements */
+  const float* noise; /* the noise image at known elements (NULL: not packed; a boundary that needs it fails) */
+} lp_known;
+
+int64_t lp_known_words(int64_t total);
+
+/* Builds words, y_known and (if noise != NULL) noise_known from the uint8 mask and the dense operands: three
+ * small launches, once per job.  Reads the mask through dims like every other entry point. */
+int lp_pack_known(const uint8_t* mask, const lp_dims* dims, const float* y, const float* noise, uint32_t* words,
+                  float* y_known, float* noise_known, lp_stream_t stream);
+
 /* Replace step + change of variables, lanpaint.py:85-99:
  *   x_model = mask ? rep_noise*noise + rep_y*y : x
  * written to x_model (may alias x) and, if non-NULL, x_copy. */
@@ -229,6 +253,13 @@ int lp_substep_f32(float* x_model, const float* x0, const float* x0_big, const f
 int lp_substep(float* x_model, const lp_heads* heads, const float* y, const uint8_t* mask, float* c_state,
                float* x_copy, float* x0e_out, const float* table, const lp_dims* dims, const lp_rng* rng,
                int flags, lp_stream_t stream);
+
+/* lp_substep with the known-operand layout of the same y and mask (lp_pack_known).  The TMA-staged torch-stream
+ * kernel then fetches the packed y and the known bits instead of the dense y and the uint8 mask; every other
+ * kernel reads the dense operands, which must stay valid.  Results are bit-identical to lp_substep. */
+int lp_substep_known(float* x_model, const lp_heads* heads, const float* y, const uint8_t* mask, const lp_known* known,
+                     float* c_state, float* x_copy, float* x0e_out, const float* table, const lp_dims* dims,
+                     const lp_rng* rng, int flags, lp_stream_t stream);
 
 /* lp_substep_f32 with the two classifier-free-guidance combines folded in (SURVEY 8f rank 1; replaces the
  * two cfg_function calls of sampling_function_LanPaint, src/LanPaint/nodes.py:175): the caller passes the
@@ -280,6 +311,13 @@ int lp_step_boundary_f32(const float* model_out, const float* y, const float* no
  * lp_epilogue_f32, lp_epilogue_euler_f32, lp_step_boundary_f32 and lp_epilogue_cfg_f32 are special cases. */
 int lp_boundary(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask, float* x_inout,
                 float* out, float euler_coef, const float* next_table, const lp_dims* dims, lp_stream_t stream);
+
+/* lp_boundary with the known-operand layout (lp_pack_known; known->noise is needed when next_table != NULL): the
+ * LDG kernel reads the known bits and the packed y / noise instead of the uint8 mask and the dense y / noise.
+ * The TMA-staged kernel (option "tma_boundary") keeps the dense operands.  Bit-identical to lp_boundary. */
+int lp_boundary_known(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                      const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
+                      const lp_dims* dims, lp_stream_t stream);
 
 /* Final denoise of an outer step straight from raw cond / uncond predictions:
  *   out = mask ? y : uncond + (cond - uncond)*cfg ;  if x_inout != NULL: x = x + (x - out)*euler_coef. */

@@ -24,7 +24,7 @@ SUBSTEP_FIRST, SUBSTEP_FUSE_NEXT, SUBSTEP_STORE_C, SUBSTEP_MERGE_NOISE = 1, 2, 4
 SYMBOLS = (
     "lp_abi_version", "lp_status_string", "lp_last_cuda_error", "lp_set_option", "lp_selftest_index_math", "lp_selftest_box_muller", "lp_build_coef_table", "lp_build_coef_table_dt",
     "lp_torch_randn_geometry", "lp_pack_mask_f32", "lp_prologue_f32", "lp_substep", "lp_substep_f32", "lp_substep_cfg_f32", "lp_advance_f32",
-    "lp_boundary", "lp_synth_denoiser",
+    "lp_boundary", "lp_synth_denoiser", "lp_known_words", "lp_pack_known", "lp_substep_known", "lp_boundary_known",
     "lp_epilogue_f32", "lp_epilogue_euler_f32", "lp_step_boundary_f32", "lp_epilogue_cfg_f32", "lp_stop_stats_f32", "lp_fill_normal_f32", "lp_synth_denoiser_f32", "lp_l2_persist_capacity", "lp_l2_persist_set", "lp_l2_persist_clear", "lp_l2_flush", "lp_torch_cpu_randn_f32",
 )
 
@@ -52,6 +52,11 @@ class Dims(C.Structure):
 class Rng(C.Structure):
     _fields_ = [("mode", C.c_int32), ("reserved", C.c_int32), ("tape0", C.c_void_p), ("tape1", C.c_void_p),
                 ("seed", C.c_uint64), ("draw0", C.c_uint64), ("draw1", C.c_uint64), ("state", C.c_void_p)]
+
+
+class Known(C.Structure):
+    """lp_known: the known-operand layout (known bits + packed y / noise) of one job's y, noise and mask."""
+    _fields_ = [("words", C.c_void_p), ("y", C.c_void_p), ("noise", C.c_void_p)]
 
 
 _lib: Optional[C.CDLL] = None
@@ -98,6 +103,15 @@ def load() -> C.CDLL:
     lib.lp_substep.argtypes = [p, C.POINTER(Heads), p, p, p, p, p, p, C.POINTER(Dims), C.POINTER(Rng), i32, p]
     lib.lp_boundary.restype = i32
     lib.lp_boundary.argtypes = [C.POINTER(Heads), p, p, p, p, p, C.c_float, p, C.POINTER(Dims), p]
+    lib.lp_known_words.restype = i64
+    lib.lp_known_words.argtypes = [i64]
+    lib.lp_pack_known.restype = i32
+    lib.lp_pack_known.argtypes = [p, C.POINTER(Dims), p, p, p, p, p, p]
+    lib.lp_substep_known.restype = i32
+    lib.lp_substep_known.argtypes = [p, C.POINTER(Heads), p, p, C.POINTER(Known), p, p, p, p, C.POINTER(Dims),
+                                     C.POINTER(Rng), i32, p]
+    lib.lp_boundary_known.restype = i32
+    lib.lp_boundary_known.argtypes = [C.POINTER(Heads), p, p, p, C.POINTER(Known), p, p, C.c_float, p, C.POINTER(Dims), p]
     lib.lp_synth_denoiser.restype = i32
     lib.lp_synth_denoiser.argtypes = [p, p, p, i32, i64, p, p]
     lib.lp_substep_f32.restype = i32

@@ -41,6 +41,9 @@ struct BoundaryArgs {
   const float* y;
   const float* noise;
   const uint8_t* mask;
+  const uint32_t* kwords;  // known-operand layout (lp_known) or NULL
+  const float* yk;         // y at known elements
+  const float* nk;         // noise at known elements
   float* x;        // NULL: no Euler update
   float* out;      // NULL: nobody reads the denoised latent
   const float* next_table;  // NULL: no replace step of the next outer step
@@ -59,26 +62,50 @@ __device__ __forceinline__ void boundary_element(float a, float b, float y, floa
   if (next) x = known ? fmaf(rn, nz, ry * y) : x;
 }
 
-template <int N, typename H>
+// kPk: the known bits and the packed y / noise of lp_known replace the uint8 mask and the dense y / noise, so y and
+// noise cost 4 B per KNOWN element each instead of 4 B per element (a 4-wide vector is rarely all-free, so the dense
+// form reads nearly all of y on a scattered mask).
+template <int N, typename H, bool kPk>
 __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) {
   pdl_prologue();
   const uint32_t i = (blockIdx.x * kBlock + threadIdx.x) * N;
   if (i >= p.g.total) return;
   uint32_t row, mi;
   locate(p.g, i, row, mi);
+  const bool euler = p.x != nullptr, next = p.next_table != nullptr;
+  float av[N], bv[N], yv[N], xv[N], nv[N], ov[N];
   bool known[N];
-  load_m<N>(p.mask, mi, known);
+  uint32_t kb = 0, kidx = 0;
+  if constexpr (kPk) {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
+    if constexpr (N == 4) {
+      known_quad(w, i, kb, kidx);
+    } else {
+      kb = (w.x >> (i & 31u)) & 1u;
+      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
+    }
+#pragma unroll
+    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
+  } else {
+    load_m<N>(p.mask, mi, known);
+  }
   bool any_known = false, any_free = false;
 #pragma unroll
   for (int j = 0; j < N; ++j) {
     any_known |= known[j];
     any_free |= !known[j];
   }
-  const bool euler = p.x != nullptr, next = p.next_table != nullptr;
-  float av[N], bv[N], yv[N], xv[N], nv[N], ov[N];
 #pragma unroll
   for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = 0.f;
-  load_f_ro<N>(p.y, i, yv);
+  if constexpr (kPk) {
+    if constexpr (N == 4) {
+      gather_known4<false>(p.yk, kb, kidx, yv);
+    } else {
+      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
+    }
+  } else {
+    load_f_ro<N>(p.y, i, yv);
+  }
   // free positions: the denoised output and the running state; known positions: the re-noised clean latent
   if (any_free) {
     load_head_ro<N, H>(static_cast<const H*>(p.a), i, av);
@@ -87,7 +114,15 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
   if (euler && (any_free || !next)) load_f<N>(p.x, i, xv);
   float rn = 0.f, ry = 0.f;
   if (next) {
-    if (any_known) load_f_ro<N>(p.noise, i, nv);
+    if constexpr (kPk) {
+      if constexpr (N == 4) {
+        gather_known4<false>(p.nk, kb, kidx, nv);
+      } else {
+        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
+      }
+    } else {
+      if (any_known) load_f_ro<N>(p.noise, i, nv);
+    }
     rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
     ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
   }
@@ -224,15 +259,21 @@ int boundary_dispatch(const BoundaryArgs& p, bool v4, int dtype, cudaStream_t s)
     if (p.next_table) return launch_boundary_tma<H, false, true>(p, s);
     return launch_boundary_tma<H, false, false>(p, s);
   }
-  if (v4) launch_kernel(boundary_kernel<4, H>, dim3(blocks_for(p.g.total / 4)), s, p);
-  else launch_kernel(boundary_kernel<1, H>, dim3(blocks_for(p.g.total)), s, p);
+  if (p.kwords) {
+    if (v4) launch_kernel(boundary_kernel<4, H, true>, dim3(blocks_for(p.g.total / 4)), s, p);
+    else launch_kernel(boundary_kernel<1, H, true>, dim3(blocks_for(p.g.total)), s, p);
+  } else {
+    if (v4) launch_kernel(boundary_kernel<4, H, false>, dim3(blocks_for(p.g.total / 4)), s, p);
+    else launch_kernel(boundary_kernel<1, H, false>, dim3(blocks_for(p.g.total)), s, p);
+  }
   return check_launch();
 }
 
-static int boundary_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask, float* x_inout,
-                         float* out, float euler_coef, const float* next_table, const lp_dims* dims,
-                         lp_stream_t stream) {
+static int boundary_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                         const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
+                         const lp_dims* dims, lp_stream_t stream) {
   if (!mo || !mo->a || !y || !mask) return LP_ERR_INVALID;
+  if (known && (!known->words || !known->y || (next_table && !known->noise))) return LP_ERR_INVALID;
   if (!x_inout && !out) return LP_ERR_INVALID;
   if (next_table && (!noise || !x_inout)) return LP_ERR_INVALID;
   const int dtype = mo->dtype;
@@ -242,6 +283,7 @@ static int boundary_impl(const lp_heads* mo, const float* y, const float* noise,
   if (int rc = make_geometry(dims, p.g)) return rc;
   if (p.g.total == 0) return LP_OK;
   p.a = mo->a; p.b = mo->combine ? mo->b : nullptr; p.y = y; p.noise = noise; p.mask = mask; p.x = x_inout; p.out = out;
+  p.kwords = known ? known->words : nullptr; p.yk = known ? known->y : nullptr; p.nk = known ? known->noise : nullptr;
   p.next_table = next_table; p.cfg = mo->cfg; p.coef = euler_coef; p.combine = mo->combine != 0;
   const bool v4 = geometry_vec4(p.g, mask) && head_aligned(p.a, dtype) && (!p.b || head_aligned(p.b, dtype)) &&
                   aligned16(y) && (!noise || aligned16(noise)) && (!x_inout || aligned16(x_inout)) &&
@@ -410,21 +452,28 @@ extern "C" int lp_prologue_f32(const float* x, const float* y, const float* nois
 extern "C" int lp_boundary(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                            float* x_inout, float* out, float euler_coef, const float* next_table, const lp_dims* dims,
                            lp_stream_t stream) {
-  return boundary_impl(model_out, y, noise, mask, x_inout, out, euler_coef, next_table, dims, stream);
+  return boundary_impl(model_out, y, noise, mask, nullptr, x_inout, out, euler_coef, next_table, dims, stream);
+}
+
+extern "C" int lp_boundary_known(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                                 const lp_known* known, float* x_inout, float* out, float euler_coef,
+                                 const float* next_table, const lp_dims* dims, lp_stream_t stream) {
+  if (!known) return LP_ERR_INVALID;
+  return boundary_impl(model_out, y, noise, mask, known, x_inout, out, euler_coef, next_table, dims, stream);
 }
 
 extern "C" int lp_epilogue_f32(const float* model_out, const float* y, const uint8_t* mask, float* out,
                                const lp_dims* dims, lp_stream_t stream) {
   if (!out) return LP_ERR_INVALID;
   lp_heads h = {model_out, nullptr, LP_DTYPE_F32, 0, 0.f, 0.f};
-  return boundary_impl(&h, y, nullptr, mask, nullptr, out, 0.f, nullptr, dims, stream);
+  return boundary_impl(&h, y, nullptr, mask, nullptr, nullptr, out, 0.f, nullptr, dims, stream);
 }
 
 extern "C" int lp_epilogue_euler_f32(const float* model_out, const float* y, const uint8_t* mask, float* x_inout,
                                      float* out, float euler_coef, const lp_dims* dims, lp_stream_t stream) {
   if (!x_inout) return LP_ERR_INVALID;
   lp_heads h = {model_out, nullptr, LP_DTYPE_F32, 0, 0.f, 0.f};
-  return boundary_impl(&h, y, nullptr, mask, x_inout, out, euler_coef, nullptr, dims, stream);
+  return boundary_impl(&h, y, nullptr, mask, nullptr, x_inout, out, euler_coef, nullptr, dims, stream);
 }
 
 extern "C" int lp_step_boundary_f32(const float* model_out, const float* y, const float* noise, const uint8_t* mask,
@@ -432,7 +481,7 @@ extern "C" int lp_step_boundary_f32(const float* model_out, const float* y, cons
                                     const lp_dims* dims, lp_stream_t stream) {
   if (!noise || !x_inout || !next_table) return LP_ERR_INVALID;
   lp_heads h = {model_out, nullptr, LP_DTYPE_F32, 0, 0.f, 0.f};
-  return boundary_impl(&h, y, noise, mask, x_inout, out, euler_coef, next_table, dims, stream);
+  return boundary_impl(&h, y, noise, mask, nullptr, x_inout, out, euler_coef, next_table, dims, stream);
 }
 
 extern "C" int lp_epilogue_cfg_f32(const float* cond, const float* uncond, float cfg, const float* y,
@@ -440,7 +489,7 @@ extern "C" int lp_epilogue_cfg_f32(const float* cond, const float* uncond, float
                                    const lp_dims* dims, lp_stream_t stream) {
   if (!cond || !uncond || !out) return LP_ERR_INVALID;
   lp_heads h = {cond, uncond, LP_DTYPE_F32, 1, cfg, cfg};
-  return boundary_impl(&h, y, nullptr, mask, x_inout, out, euler_coef, nullptr, dims, stream);
+  return boundary_impl(&h, y, nullptr, mask, nullptr, x_inout, out, euler_coef, nullptr, dims, stream);
 }
 
 extern "C" int lp_advance_f32(float* x_model, const float* c_state, const uint8_t* mask, const float* table,

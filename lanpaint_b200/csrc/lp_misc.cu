@@ -104,6 +104,90 @@ __global__ void __launch_bounds__(kBlock) pack_mask_kernel(const float* __restri
   out[i] = (hi != (invert != 0)) ? 1 : 0;
 }
 
+// ---- the known-operand layout (lp_known): three launches, once per job -------------------------------------
+// Words are handled in blocks of kBlock; words[2W..2W+1] is the end sentinel {0, known count}, and the tail of the
+// buffer holds one count per block of words for the scan.
+inline uint32_t known_word_count(uint32_t total) { return (total + 31u) / 32u + 1u; }  // W + the sentinel
+
+// Inclusive prefix sum over the kBlock threads of a block (Hillis-Steele in shared memory).
+__device__ __forceinline__ uint32_t block_inclusive_sum(uint32_t v, uint32_t* s) {
+  s[threadIdx.x] = v;
+  __syncthreads();
+#pragma unroll
+  for (int o = 1; o < kBlock; o <<= 1) {
+    const uint32_t add = threadIdx.x >= (uint32_t)o ? s[threadIdx.x - o] : 0u;
+    __syncthreads();
+    s[threadIdx.x] += add;
+    __syncthreads();
+  }
+  return s[threadIdx.x];
+}
+
+// words[2w] = known bits of elements 32w..32w+31 (through the mask's strides); block_sums[b] = known elements of
+// word block b
+__global__ void __launch_bounds__(kBlock) known_bits_kernel(const uint8_t* __restrict__ mask, Geometry g,
+                                                            uint32_t* words, uint32_t* block_sums, uint32_t n_words) {
+  __shared__ uint32_t s[kBlock];
+  pdl_prologue();
+  const uint32_t w = blockIdx.x * kBlock + threadIdx.x;
+  uint32_t bits = 0;
+  if (w < n_words) {
+    for (uint32_t b = 0; b < 32u; ++b) {
+      const uint32_t e = 32u * w + b;
+      if (e >= g.total) break;
+      uint32_t row, mi;
+      locate(g, e, row, mi);
+      bits |= (__ldg(mask + mi) != 0 ? 1u : 0u) << b;
+    }
+    words[2u * w] = bits;
+  }
+  const uint32_t sum = block_inclusive_sum(__popc(bits), s);
+  if (threadIdx.x == kBlock - 1) block_sums[blockIdx.x] = sum;
+}
+
+// block_sums -> their exclusive prefix sums, in place (one CTA)
+__global__ void __launch_bounds__(kBlock) known_scan_kernel(uint32_t* block_sums, uint32_t n_blocks) {
+  __shared__ uint32_t s[kBlock];
+  pdl_prologue();
+  uint32_t carry = 0;
+  for (uint32_t base = 0; base < n_blocks; base += kBlock) {
+    const uint32_t i = base + threadIdx.x;
+    const uint32_t v = i < n_blocks ? block_sums[i] : 0u;
+    const uint32_t inc = block_inclusive_sum(v, s);
+    if (i < n_blocks) block_sums[i] = carry + inc - v;
+    carry += s[kBlock - 1];
+    __syncthreads();
+  }
+}
+
+// words[2w + 1] = known elements before 32w; then every known element's y (and noise) to its packed index
+__global__ void __launch_bounds__(kBlock) known_scatter_kernel(uint32_t* words, const uint32_t* __restrict__ block_sums,
+                                                               uint32_t n_words, uint32_t total,
+                                                               const float* __restrict__ y,
+                                                               const float* __restrict__ noise, float* yk, float* nk) {
+  __shared__ uint32_t s[kBlock], sbits[kBlock], sbase[kBlock];
+  pdl_prologue();
+  const uint32_t w = blockIdx.x * kBlock + threadIdx.x;
+  const uint32_t bits = w < n_words ? words[2u * w] : 0u;
+  const uint32_t c = __popc(bits);
+  const uint32_t base = block_sums[blockIdx.x] + block_inclusive_sum(c, s) - c;
+  if (w < n_words) words[2u * w + 1u] = base;
+  sbits[threadIdx.x] = bits;
+  sbase[threadIdx.x] = base;
+  __syncthreads();
+  const uint32_t e0 = blockIdx.x * kBlock * 32u;
+  const uint32_t e1 = e0 >= total ? e0 : (total - e0 < kBlock * 32u ? total : e0 + kBlock * 32u);
+  for (uint32_t e = e0 + threadIdx.x; e < e1; e += kBlock) {
+    const uint32_t wl = (e - e0) >> 5, b = e & 31u;
+    const uint32_t m = sbits[wl];
+    if ((m >> b) & 1u) {
+      const uint32_t idx = sbase[wl] + __popc(m & ((1u << b) - 1u));
+      yk[idx] = __ldg(y + e);
+      if (nk) nk[idx] = __ldg(noise + e);
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kBlock) fill_normal_philox_kernel(float* out, uint32_t n, uint64_t seed,
                                                                     uint64_t draw, const uint64_t* st) {
   pdl_prologue();
@@ -280,6 +364,28 @@ extern "C" int lp_pack_mask_f32(const float* mask_f32, uint8_t* mask_u8, int64_t
   if (n == 0) return LP_OK;
   launch_kernel(pack_mask_kernel, dim3(blocks_for((uint32_t)n)), (cudaStream_t)stream, mask_f32, mask_u8,
                                                                                  (uint32_t)n, invert);
+  return check_launch();
+}
+
+extern "C" int64_t lp_known_words(int64_t total) {
+  if (total < 0 || total >= (int64_t(1) << 31)) return -1;
+  const int64_t n_words = known_word_count((uint32_t)total);
+  return 2 * n_words + (n_words + kBlock - 1) / kBlock;
+}
+
+extern "C" int lp_pack_known(const uint8_t* mask, const lp_dims* dims, const float* y, const float* noise,
+                             uint32_t* words, float* y_known, float* noise_known, lp_stream_t stream) {
+  if (!mask || !y || !words || !y_known || (noise && !noise_known)) return LP_ERR_INVALID;
+  Geometry g;
+  if (int rc = make_geometry(dims, g)) return rc;
+  const uint32_t n_words = known_word_count(g.total);
+  const uint32_t n_blocks = (n_words + kBlock - 1) / kBlock;
+  uint32_t* block_sums = words + 2u * n_words;
+  cudaStream_t s = (cudaStream_t)stream;
+  launch_kernel(known_bits_kernel, dim3(n_blocks), s, mask, g, words, block_sums, n_words);
+  launch_kernel(known_scan_kernel, dim3(1), s, block_sums, n_blocks);
+  launch_kernel(known_scatter_kernel, dim3(n_blocks), s, words, (const uint32_t*)block_sums, n_words, g.total, y,
+                noise, y_known, noise ? noise_known : nullptr);
   return check_launch();
 }
 

@@ -20,6 +20,8 @@ struct SubstepArgs {
   const void* x0b;
   const float* y;
   const uint8_t* mask;
+  const uint32_t* kwords;  // known-operand layout (lp_known) or NULL: dense y and mask only
+  const float* yk;         // y at known elements
   float* c;
   float* x_copy;
   float* x0e;
@@ -261,12 +263,19 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) substep_tma_kernel(const S
 //   * consumer thread c owns subsequences 4c..4c+3 of the block: 4 Philox calls per draw, cuRAND's exact
 //     Box-Muller, and its four normals per plane are one float4 of that plane's sub-tile -- no shuffles.
 // Same Philox stream, same arithmetic as the LDG kernels: bit-identical results.
-template <typename H, int kG>
+//
+// kPk: the known-operand layout (lp_known).  A sub-tile starts on a multiple of 1024 elements, so its known bits
+// are 32 whole words and its known y values one contiguous packed span; the producer fetches the words and that
+// span, widened to 16-byte bounds, in place of the dense y slice and the uint8 mask slices (4 B/element of y
+// become 4 B per KNOWN element; 1 B/element of mask staging becomes 1/4).  A consumer finds its four y values at
+// word.base + popc(word.bits & below) in the staged span.
+template <typename H, int kG, bool kPk>
 struct __align__(128) TorchSlot {
   float x[kG];
   H x0[kG], x0b[kG];
-  float y[kG], c[kG];
-  uint8_t m[kG];
+  float y[kPk ? kG + 8 : kG], c[kG];
+  uint8_t m[kPk ? 16 : kG];   // every member starts on a 16-byte boundary (cp.async.bulk destinations)
+  uint2 w[kPk ? kG / 32 : 2];
 };
 
 struct TorchTmaGeom {
@@ -275,11 +284,11 @@ struct TorchTmaGeom {
 };
 
 // kG subsequences per group = 4 per consumer thread; one extra warp produces.
-template <typename H, bool kFirst, bool kNext, int kG>
+template <typename H, bool kFirst, bool kNext, int kG, bool kPk>
 __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const TorchTmaGeom& tg, unsigned char* smem_raw,
                                                uint64_t* full, uint64_t* empty) {
   constexpr int kConsumers = kG / 4;
-  using Slot = TorchSlot<H, kG>;
+  using Slot = TorchSlot<H, kG, kPk>;
   Slot* slot = reinterpret_cast<Slot*>(smem_raw);
   pdl_prologue();
   const uint32_t T = a.torch_T, total = a.g.total;
@@ -314,34 +323,62 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
       uint32_t it = 0;
       for (uint32_t grp = blockIdx.x; grp < tg.n_groups; grp += gridDim.x, ++it) {
         const uint32_t k = grp / tg.groups_per_call, b = grp - k * tg.groups_per_call;
+        uint32_t lo[4] = {0u, 0u, 0u, 0u}, hi[4] = {0u, 0u, 0u, 0u};
+        if constexpr (kPk) {  // the packed-y spans of the group: loaded before the first slot wait, which hides them
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            uint32_t e0, len;
+            subtile(k, b, j, e0, len);
+            if (len) {
+              lo[j] = __ldg(a.kwords + 2u * (e0 >> 5) + 1u);
+              hi[j] = __ldg(a.kwords + 2u * ((e0 + len + 31u) >> 5) + 1u);
+            }
+          }
+        }
 #pragma unroll 1
         for (int j = 0; j < 4; ++j) {
           mbar_wait_relaxed(&empty[j], (it & 1u) ^ 1u);  // consumers have drained this slot (passes at once the first time)
           uint32_t e0, len;
           subtile(k, b, j, e0, len);
           const uint32_t fb = len * 4u, hb = len * (uint32_t)sizeof(H);
-          // an empty sub-tile (past the end of the tensor) still completes its phase: expect 0 bytes
-          mbar_expect_tx(&full[j], fb * (2u + (kFirst ? 0u : 1u)) + hb * (1u + (aliased ? 0u : 1u)) + len);
-          if (len == 0) continue;
+          const uint32_t heads = hb * (1u + (aliased ? 0u : 1u));
           Slot& t = slot[j];
-          tma_load_1d(t.x, a.x + e0, fb, &full[j]);
-          tma_load_1d(t.x0, x0p + e0, hb, &full[j]);
-          if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j]);
-          tma_load_1d(t.y, a.y + e0, fb, &full[j]);
-          if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j]);
-          // the mask is indexed per (row, channel): one slice per channel segment the sub-tile touches
-          uint32_t e = e0, off = 0, rem = len;
-          while (rem) {
-            const uint32_t row = a.g.per_row.div(e);
-            const uint32_t r = e - row * a.g.per_row.d;
-            const uint32_t ch = a.g.spatial.div(r);
-            const uint32_t s = r - ch * a.g.spatial.d;
-            const uint32_t seg = rem < a.g.spatial.d - s ? rem : a.g.spatial.d - s;
-            tma_load_1d(t.m + off, a.mask + row * a.g.mask_row_stride + ch * a.g.mask_channel_stride + s, seg,
-                        &full[j]);
-            e += seg;
-            off += seg;
-            rem -= seg;
+          if constexpr (kPk) {
+            const uint32_t nw = (((len + 31u) >> 5) + 1u) & ~1u;  // whole words, an even number: 16-byte multiple
+            const uint32_t ylo = (j == 0 ? lo[0] : j == 1 ? lo[1] : j == 2 ? lo[2] : lo[3]) & ~3u;
+            const uint32_t yhi = ((j == 0 ? hi[0] : j == 1 ? hi[1] : j == 2 ? hi[2] : hi[3]) + 3u) & ~3u;
+            const uint32_t yb = (yhi - ylo) * 4u;
+            // an empty sub-tile (past the end of the tensor) still completes its phase: expect 0 bytes
+            mbar_expect_tx(&full[j], len ? fb * (1u + (kFirst ? 0u : 1u)) + heads + yb + nw * 8u : 0u);
+            if (len == 0) continue;
+            tma_load_1d(t.x, a.x + e0, fb, &full[j]);
+            tma_load_1d(t.x0, x0p + e0, hb, &full[j]);
+            if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j]);
+            if (yb) tma_load_1d(t.y, a.yk + ylo, yb, &full[j]);
+            if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j]);
+            tma_load_1d(t.w, a.kwords + 2u * (e0 >> 5), nw * 8u, &full[j]);
+          } else {
+            mbar_expect_tx(&full[j], fb * (2u + (kFirst ? 0u : 1u)) + heads + len);
+            if (len == 0) continue;
+            tma_load_1d(t.x, a.x + e0, fb, &full[j]);
+            tma_load_1d(t.x0, x0p + e0, hb, &full[j]);
+            if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j]);
+            tma_load_1d(t.y, a.y + e0, fb, &full[j]);
+            if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j]);
+            // the mask is indexed per (row, channel): one slice per channel segment the sub-tile touches
+            uint32_t e = e0, off = 0, rem = len;
+            while (rem) {
+              const uint32_t row = a.g.per_row.div(e);
+              const uint32_t r = e - row * a.g.per_row.d;
+              const uint32_t ch = a.g.spatial.div(r);
+              const uint32_t s = r - ch * a.g.spatial.d;
+              const uint32_t seg = rem < a.g.spatial.d - s ? rem : a.g.spatial.d - s;
+              tma_load_1d(t.m + off, a.mask + row * a.g.mask_row_stride + ch * a.g.mask_channel_stride + s, seg,
+                          &full[j]);
+              e += seg;
+              off += seg;
+              rem -= seg;
+            }
           }
         }
       }
@@ -359,7 +396,7 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
   const uint32_t tid = threadIdx.x;  // vector index inside every sub-tile
   // everything a thread does with one sub-tile once its data is in registers
   auto finish = [&](uint32_t i, float (&x)[4], float (&x0)[4], float (&x0b)[4], const float (&y)[4],
-                    const float (&cp)[4], uchar4 mv, const float2 (&p1)[4], const float2 (&p2)[4], int jj) {
+                    const float (&cp)[4], uint32_t kb, const float2 (&p1)[4], const float2 (&p2)[4], int jj) {
     const uint32_t row = a.g.per_row.div(i);
     RowCoef<kFirst, kNext> rc;
     rc.load(a.table + (size_t)row * LP_TABLE_STRIDE);
@@ -367,7 +404,7 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
 #pragma unroll
       for (int q = 0; q < 4; ++q) cfg_combine(x0[q], x0b[q], a.cfg, a.cfg_big);
     }
-    const bool known[4] = {mv.x != 0, mv.y != 0, mv.z != 0, mv.w != 0};
+    const bool known[4] = {(kb & 1u) != 0, (kb & 2u) != 0, (kb & 4u) != 0, (kb & 8u) != 0};
     float cn[4];
 #pragma unroll
     for (int q = 0; q < 4; q += 2) {   // two elements per lane-pair op; bit-identical to substep_element
@@ -384,7 +421,7 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
     if (kNext || a.store_c) *reinterpret_cast<float4*>(a.c + i) = make_float4(cn[0], cn[1], cn[2], cn[3]);
   };
   auto fetch = [&](const Slot& t, float (&x)[4], float (&x0)[4], float (&x0b)[4], float (&y)[4], float (&cp)[4],
-                   uchar4& mv) {
+                   uint32_t& kb) {
     const float4 xv = reinterpret_cast<const float4*>(t.x)[tid];
     lds_head4<H>(t.x0, tid, x0);
     if (aliased) {
@@ -393,11 +430,18 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
     } else {
       lds_head4<H>(t.x0b, tid, x0b);
     }
-    const float4 yv = reinterpret_cast<const float4*>(t.y)[tid];
+    if constexpr (kPk) {
+      uint32_t idx;
+      known_quad(t.w[tid >> 3], 4u * tid, kb, idx);
+      gather_known4<true>(t.y, kb, idx - (t.w[0].y & ~3u), y);  // the span starts at the first word's base, rounded down
+    } else {
+      const float4 yv = reinterpret_cast<const float4*>(t.y)[tid];
+      const uchar4 mv = reinterpret_cast<const uchar4*>(t.m)[tid];
+      y[0] = yv.x; y[1] = yv.y; y[2] = yv.z; y[3] = yv.w;
+      kb = (mv.x != 0 ? 1u : 0u) | (mv.y != 0 ? 2u : 0u) | (mv.z != 0 ? 4u : 0u) | (mv.w != 0 ? 8u : 0u);
+    }
     const float4 cv = kFirst ? make_float4(0.f, 0.f, 0.f, 0.f) : reinterpret_cast<const float4*>(t.c)[tid];
-    mv = reinterpret_cast<const uchar4*>(t.m)[tid];
     x[0] = xv.x; x[1] = xv.y; x[2] = xv.z; x[3] = xv.w;
-    y[0] = yv.x; y[1] = yv.y; y[2] = yv.z; y[3] = yv.w;
     cp[0] = cv.x; cp[1] = cv.y; cp[2] = cv.z; cp[3] = cv.w;
   };
   // every consumer THREAD releases the slot itself once its reads are in registers.  (One arrive per warp after a
@@ -434,193 +478,32 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
       for (int jj = 0; jj < 2; ++jj) {
         const int j = 2 * h + jj;
         float x[4], x0[4], x0b[4], y[4], cp[4];
-        uchar4 mv = make_uchar4(0, 0, 0, 0);
+        uint32_t kb = 0;
         mbar_wait(&full[j], it & 1u);
         if (whole) {
-          fetch(slot[j], x, x0, x0b, y, cp, mv);
+          fetch(slot[j], x, x0, x0b, y, cp, kb);
           release(j);  // this warp's reads of slot j are in registers: let it refill
-          finish((4u * k + (uint32_t)j) * T + t0, x, x0, x0b, y, cp, mv, p1, p2, jj);
+          finish((4u * k + (uint32_t)j) * T + t0, x, x0, x0b, y, cp, kb, p1, p2, jj);
         } else {
           uint32_t e0, len;
           subtile(k, b, j, e0, len);
           const bool active = 4u * tid < len;
-          if (active) fetch(slot[j], x, x0, x0b, y, cp, mv);
+          if (active) fetch(slot[j], x, x0, x0b, y, cp, kb);
           release(j);
-          if (active) finish(e0 + 4u * tid, x, x0, x0b, y, cp, mv, p1, p2, jj);
+          if (active) finish(e0 + 4u * tid, x, x0, x0b, y, cp, kb, p1, p2, jj);
         }
       }
     }
   }
 }
 
-// ---- the same kernel with TWO subsequences per consumer thread ---------------------------------------------------
-// Half the per-thread state (2 Philox calls per draw, one lane-pair Box-Muller call per draw and half, one lane-pair
-// update per plane, LDS.64 / STG.64), so the register ceiling can drop to 64 and twice as many consumer warps fit per SM:
-// the kernel is bound by issue latency, not by the pipes.  Groups of kG subsequences need not divide T.
-template <typename H, bool kFirst, bool kNext, int kG>
-__device__ __forceinline__ void torch_tma_body2(const SubstepArgs& a, const TorchTmaGeom& tg, unsigned char* smem_raw,
-                                                uint64_t* full, uint64_t* empty) {
-  constexpr int kConsumers = kG / 2;
-  using Slot = TorchSlot<H, kG>;
-  Slot* slot = reinterpret_cast<Slot*>(smem_raw);
-  pdl_prologue();
-  const uint32_t T = a.torch_T, total = a.g.total;
-  const bool aliased = a.x0b == a.x0;
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      mbar_init(&full[j], 1);
-      mbar_init(&empty[j], kConsumers);
-    }
-    mbar_fence_init();
-  }
-  __syncthreads();
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // first element / length of sub-tile j of group (k, b): clipped by the end of the plane and of the tensor
-  auto subtile = [&](uint32_t k, uint32_t b, int j, uint32_t& e0, uint32_t& len) {
-    const uint32_t in_plane = T - b * kG < (uint32_t)kG ? T - b * kG : (uint32_t)kG;
-    const uint64_t e = (uint64_t)(4u * k + (uint32_t)j) * T + (uint64_t)b * kG;
-    if (e >= total) {
-      e0 = 0;
-      len = 0;
-    } else {
-      e0 = (uint32_t)e;
-      len = total - e0 < in_plane ? total - e0 : in_plane;
-    }
-  };
-
-  if (warp == kConsumers / 32) {  // ---------------- producer ----------------
-    if (lane == 0) {
-      const H* x0p = static_cast<const H*>(a.x0);
-      const H* x0bp = static_cast<const H*>(a.x0b);
-      uint32_t it = 0;
-      for (uint32_t grp = blockIdx.x; grp < tg.n_groups; grp += gridDim.x, ++it) {
-        const uint32_t k = grp / tg.groups_per_call, b = grp - k * tg.groups_per_call;
-#pragma unroll 1
-        for (int j = 0; j < 4; ++j) {
-          mbar_wait_relaxed(&empty[j], (it & 1u) ^ 1u);
-          uint32_t e0, len;
-          subtile(k, b, j, e0, len);
-          const uint32_t fb = len * 4u, hb = len * (uint32_t)sizeof(H);
-          mbar_expect_tx(&full[j], fb * (2u + (kFirst ? 0u : 1u)) + hb * (1u + (aliased ? 0u : 1u)) + len);
-          if (len == 0) continue;
-          Slot& t = slot[j];
-          tma_load_1d(t.x, a.x + e0, fb, &full[j]);
-          tma_load_1d(t.x0, x0p + e0, hb, &full[j]);
-          if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j]);
-          tma_load_1d(t.y, a.y + e0, fb, &full[j]);
-          if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j]);
-          uint32_t e = e0, off = 0, rem = len;
-          while (rem) {
-            const uint32_t row = a.g.per_row.div(e);
-            const uint32_t r = e - row * a.g.per_row.d;
-            const uint32_t ch = a.g.spatial.div(r);
-            const uint32_t s = r - ch * a.g.spatial.d;
-            const uint32_t seg = rem < a.g.spatial.d - s ? rem : a.g.spatial.d - s;
-            tma_load_1d(t.m + off, a.mask + row * a.g.mask_row_stride + ch * a.g.mask_channel_stride + s, seg,
-                        &full[j]);
-            e += seg;
-            off += seg;
-            rem -= seg;
-          }
-        }
-      }
-    }
-    return;
-  }
-
-  // ---------------- consumers ----------------
-  uint64_t seed = a.seed, o0 = a.draw0, o1 = a.draw1;
-  if (a.rng_state) {
-    seed = a.rng_state[0];
-    o0 += a.rng_state[1];
-    o1 += a.rng_state[1];
-  }
-  const uint32_t tid = threadIdx.x;  // pair index inside every sub-tile
-  uint32_t it = 0;
-  for (uint32_t grp = blockIdx.x; grp < tg.n_groups; grp += gridDim.x, ++it) {
-    const uint32_t k = grp / tg.groups_per_call, b = grp - k * tg.groups_per_call;
-    const uint32_t t0 = b * kG + 2u * tid;  // my two Philox subsequences (torch threads)
-    const uint4 ra0 = torch_philox(seed, o0, t0, k), ra1 = torch_philox(seed, o0, t0 + 1u, k);
-    uint4 rb0 = make_uint4(0u, 0u, 0u, 0u), rb1 = rb0;
-    if (kNext) {
-      rb0 = torch_philox(seed, o1, t0, k);
-      rb1 = torch_philox(seed, o1, t0 + 1u, k);
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {  // curand_normal4: planes 0,1 <- (x,y), planes 2,3 <- (z,w)
-      float2 p1[2], p2[2];
-      box_muller_curand_x2(h ? ra0.z : ra0.x, h ? ra0.w : ra0.y, h ? ra1.z : ra1.x, h ? ra1.w : ra1.y, p1[0], p1[1]);
-      if (kNext) {
-        box_muller_curand_x2(h ? rb0.z : rb0.x, h ? rb0.w : rb0.y, h ? rb1.z : rb1.x, h ? rb1.w : rb1.y, p2[0], p2[1]);
-      } else {
-        p2[0] = p2[1] = make_float2(0.f, 0.f);
-      }
-#pragma unroll
-      for (int jj = 0; jj < 2; ++jj) {
-        const int j = 2 * h + jj;
-        uint32_t e0, len;
-        subtile(k, b, j, e0, len);
-        mbar_wait(&full[j], it & 1u);
-        const bool active = 2u * tid < len;
-        float x[2] = {0.f, 0.f}, x0[2] = {0.f, 0.f}, x0b[2] = {0.f, 0.f}, y[2] = {0.f, 0.f}, cp[2] = {0.f, 0.f};
-        uchar2 mv = make_uchar2(0, 0);
-        if (active) {
-          const Slot& t = slot[j];
-          const float2 xv = reinterpret_cast<const float2*>(t.x)[tid];
-          lds_head2<H>(t.x0, tid, x0);
-          if (aliased) {
-            x0b[0] = x0[0];
-            x0b[1] = x0[1];
-          } else {
-            lds_head2<H>(t.x0b, tid, x0b);
-          }
-          const float2 yv = reinterpret_cast<const float2*>(t.y)[tid];
-          const float2 cv = kFirst ? make_float2(0.f, 0.f) : reinterpret_cast<const float2*>(t.c)[tid];
-          mv = reinterpret_cast<const uchar2*>(t.m)[tid];
-          x[0] = xv.x; x[1] = xv.y;
-          y[0] = yv.x; y[1] = yv.y;
-          cp[0] = cv.x; cp[1] = cv.y;
-        }
-        mbar_arrive(&empty[j]);  // my reads of slot j are in registers
-        if (active) {
-          const uint32_t i = e0 + 2u * tid;
-          const uint32_t row = a.g.per_row.div(i);
-          RowCoef<kFirst, kNext> rc;
-          rc.load(a.table + (size_t)row * LP_TABLE_STRIDE);
-          if (a.use_cfg) {
-            cfg_combine(x0[0], x0b[0], a.cfg, a.cfg_big);
-            cfg_combine(x0[1], x0b[1], a.cfg, a.cfg_big);
-          }
-          const bool known[2] = {mv.x != 0, mv.y != 0};
-          const float n1[2] = {jj ? p1[0].y : p1[0].x, jj ? p1[1].y : p1[1].x};
-          const float n2[2] = {jj ? p2[0].y : p2[0].x, jj ? p2[1].y : p2[1].x};
-          float cn[2];
-          substep_element_x2<kFirst, kNext>(x, x0, x0b, y, cp, known, n1, n2, rc, cn);
-          *reinterpret_cast<float2*>(a.x + i) = make_float2(x[0], x[1]);
-          if (kNext || a.store_c) *reinterpret_cast<float2*>(a.c + i) = make_float2(cn[0], cn[1]);
-        }
-      }
-    }
-  }
-}
-
-// <448 subsequences per group, 224 consumer threads + producer warp = 256 threads, up to 4 CTAs per SM, 64 registers>.
-// Bit-identical to the default geometry; an alternative geometry, selectable with lp_set_option("tma", 8).
-template <typename H, bool kFirst, bool kNext>
-__global__ void __launch_bounds__(448 / 2 + 32, 4) substep_torch_tma_kernel_p2(const SubstepArgs a, const TorchTmaGeom tg) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full[4], empty[4];
-  torch_tma_body2<H, kFirst, kNext, 448>(a, tg, smem_raw, full, empty);
-}
-// The default geometry: <1024 subsequences per group, 256 consumer threads + producer warp, 2 CTAs per SM, 96
-// registers; 4 slots of 21 KB (fp32 heads) = 84 KB of shared memory per CTA, 168 KB per SM>.
-template <typename H, bool kFirst, bool kNext>
+// <1024 subsequences per group, 256 consumer threads + producer warp, 2 CTAs per SM, 96 registers; 4 slots of 21 KB
+// (fp32 heads) = 84 KB of shared memory per CTA, 168 KB per SM>.
+template <typename H, bool kFirst, bool kNext, bool kPk>
 __global__ void __launch_bounds__(1024 / 4 + 32, 2) substep_torch_tma_kernel(const SubstepArgs a, const TorchTmaGeom tg) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ __align__(8) uint64_t full[4], empty[4];
-  torch_tma_body<H, kFirst, kNext, 1024>(a, tg, smem_raw, full, empty);
+  torch_tma_body<H, kFirst, kNext, 1024, kPk>(a, tg, smem_raw, full, empty);
 }
 
 // ---- TORCH, 128-bit LDG path ----------------------------------------------------------------------
@@ -790,32 +673,25 @@ int launch_substep_vec(const SubstepArgs& a, bool first, bool next, bool merge, 
   return check_launch();
 }
 
-template <typename H, bool kFirst, bool kNext>
-int launch_torch_tma(const SubstepArgs& a, uint32_t calls, cudaStream_t s) {
+template <typename H, bool kFirst, bool kNext, bool kPk>
+int launch_torch_tma_cfg(const SubstepArgs& a, uint32_t calls, cudaStream_t s) {
   const int dev = current_device();
-  const int variant = (sizeof(H) == 4 && !kFirst && kNext) ? g_opt_tma : 1;   // the alternative: steady fp32 kernel only
-  if (variant == 8) {   // two subsequences per thread, groups of 448 (need not divide T)
-    const size_t smem = sizeof(TorchSlot<H, 448>) * 4;
-    TorchTmaGeom tg;
-    tg.groups_per_call = (a.torch_T + 447u) / 448u;
-    tg.n_groups = calls * tg.groups_per_call;
-    unsigned grid = (unsigned)device_info(dev).sms * 4u;
-    if (grid > tg.n_groups) grid = tg.n_groups;
-    static bool configured[kMaxDevices] = {};
-    ensure_dynamic_smem(substep_torch_tma_kernel_p2<H, kFirst, kNext>, smem, dev, configured);
-    launch_kernel_ex(substep_torch_tma_kernel_p2<H, kFirst, kNext>, dim3(grid), dim3(448 / 2 + 32), smem, s, a, tg);
-    return check_launch();
-  }
-  const size_t smem = sizeof(TorchSlot<H, 1024>) * 4;
+  const size_t smem = sizeof(TorchSlot<H, 1024, kPk>) * 4;
   TorchTmaGeom tg;
   tg.groups_per_call = a.torch_T / 1024;
   tg.n_groups = calls * tg.groups_per_call;
   unsigned grid = (unsigned)device_info(dev).sms * 2u;
   if (grid > tg.n_groups) grid = tg.n_groups;
   static bool configured[kMaxDevices] = {};
-  ensure_dynamic_smem(substep_torch_tma_kernel<H, kFirst, kNext>, smem, dev, configured);
-  launch_kernel_ex(substep_torch_tma_kernel<H, kFirst, kNext>, dim3(grid), dim3(1024 / 4 + 32), smem, s, a, tg);
+  ensure_dynamic_smem(substep_torch_tma_kernel<H, kFirst, kNext, kPk>, smem, dev, configured);
+  launch_kernel_ex(substep_torch_tma_kernel<H, kFirst, kNext, kPk>, dim3(grid), dim3(1024 / 4 + 32), smem, s, a, tg);
   return check_launch();
+}
+
+template <typename H, bool kFirst, bool kNext>
+int launch_torch_tma(const SubstepArgs& a, uint32_t calls, cudaStream_t s) {
+  return a.kwords ? launch_torch_tma_cfg<H, kFirst, kNext, true>(a, calls, s)
+                  : launch_torch_tma_cfg<H, kFirst, kNext, false>(a, calls, s);
 }
 
 template <typename H>
@@ -858,10 +734,11 @@ int substep_dispatch(SubstepArgs& a, const lp_rng* rng, bool f, bool n, bool mer
   return LP_ERR_INVALID;
 }
 
-static int substep_impl(float* x_model, const lp_heads* heads, const float* y, const uint8_t* mask, float* c_state,
-                        float* x_copy, float* x0e_out, const float* table, const lp_dims* dims, const lp_rng* rng,
-                        int flags, lp_stream_t stream) {
+static int substep_impl(float* x_model, const lp_heads* heads, const float* y, const uint8_t* mask,
+                        const lp_known* known, float* c_state, float* x_copy, float* x0e_out, const float* table,
+                        const lp_dims* dims, const lp_rng* rng, int flags, lp_stream_t stream) {
   if (!x_model || !heads || !heads->a || !y || !mask || !table || !rng) return LP_ERR_INVALID;
+  if (known && (!known->words || !known->y)) return LP_ERR_INVALID;
   if (flags & ~(LP_SUBSTEP_FIRST | LP_SUBSTEP_FUSE_NEXT | LP_SUBSTEP_STORE_C | LP_SUBSTEP_MERGE_NOISE))
     return LP_ERR_INVALID;
   const int dtype = heads->dtype;
@@ -878,6 +755,8 @@ static int substep_impl(float* x_model, const lp_heads* heads, const float* y, c
   if (int rc = make_geometry(dims, a.g)) return rc;
   if (a.g.total == 0) return LP_OK;
   a.x = x_model; a.x0 = x0; a.x0b = x0_big; a.y = y; a.mask = mask; a.c = c_state;
+  a.kwords = known && aligned16(known->words) && aligned16(known->y) ? known->words : nullptr;
+  a.yk = known ? known->y : nullptr;
   a.x_copy = x_copy; a.x0e = x0e_out; a.table = table;
   a.tape0 = rng->tape0; a.tape1 = rng->tape1; a.rng_state = rng->state;
   a.seed = rng->seed; a.draw0 = rng->draw0; a.draw1 = rng->draw1; a.torch_T = 0;
@@ -901,7 +780,15 @@ using namespace lp;
 extern "C" int lp_substep(float* x_model, const lp_heads* heads, const float* y, const uint8_t* mask, float* c_state,
                           float* x_copy, float* x0e_out, const float* table, const lp_dims* dims, const lp_rng* rng,
                           int flags, lp_stream_t stream) {
-  return substep_impl(x_model, heads, y, mask, c_state, x_copy, x0e_out, table, dims, rng, flags, stream);
+  return substep_impl(x_model, heads, y, mask, nullptr, c_state, x_copy, x0e_out, table, dims, rng, flags, stream);
+}
+
+extern "C" int lp_substep_known(float* x_model, const lp_heads* heads, const float* y, const uint8_t* mask,
+                                const lp_known* known, float* c_state, float* x_copy, float* x0e_out,
+                                const float* table, const lp_dims* dims, const lp_rng* rng, int flags,
+                                lp_stream_t stream) {
+  if (!known) return LP_ERR_INVALID;
+  return substep_impl(x_model, heads, y, mask, known, c_state, x_copy, x0e_out, table, dims, rng, flags, stream);
 }
 
 extern "C" int lp_substep_f32(float* x_model, const float* x0, const float* x0_big, const float* y,
@@ -909,7 +796,7 @@ extern "C" int lp_substep_f32(float* x_model, const float* x0, const float* x0_b
                               const float* table, const lp_dims* dims, const lp_rng* rng, int flags,
                               lp_stream_t stream) {
   lp_heads h = {x0, x0_big, LP_DTYPE_F32, 0, 0.f, 0.f};
-  return substep_impl(x_model, &h, y, mask, c_state, x_copy, x0e_out, table, dims, rng, flags, stream);
+  return substep_impl(x_model, &h, y, mask, nullptr, c_state, x_copy, x0e_out, table, dims, rng, flags, stream);
 }
 
 extern "C" int lp_substep_cfg_f32(float* x_model, const float* cond, const float* uncond, float cfg, float cfg_big,
@@ -917,5 +804,5 @@ extern "C" int lp_substep_cfg_f32(float* x_model, const float* cond, const float
                                   float* x0e_out, const float* table, const lp_dims* dims, const lp_rng* rng,
                                   int flags, lp_stream_t stream) {
   lp_heads h = {cond, uncond, LP_DTYPE_F32, 1, cfg, cfg_big};
-  return substep_impl(x_model, &h, y, mask, c_state, x_copy, x0e_out, table, dims, rng, flags, stream);
+  return substep_impl(x_model, &h, y, mask, nullptr, c_state, x_copy, x0e_out, table, dims, rng, flags, stream);
 }

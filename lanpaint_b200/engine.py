@@ -88,12 +88,51 @@ class CfgPair:
 
 
 class PackedMask:
-    """uint8 known-region mask + the strides the kernels index it with."""
+    """uint8 known-region mask + the strides the kernels index it with.  `known`, when set, is the known-operand
+    layout (`KnownOperands`) of this mask and one job's y and noise: the launches of that job then read the packed
+    operands where a kernel can (`pack_known`)."""
 
     def __init__(self, data: torch.Tensor, row_stride: int, channel_stride: int):
         self.data = data
         self.row_stride = row_stride
         self.channel_stride = channel_stride
+        self.known = None
+
+
+class KnownOperands:
+    """The known-operand layout of lp_known (include/lanpaint_b200.h): per 32 latent elements one word of known
+    bits and one count of the known elements before them, plus y and the noise image at known elements only.
+    y and the noise image are read only at known positions and are constant for a job, so a kernel that streams
+    them reads 4 B per known element instead of 4 B per element.  Buffers are sized for `total` elements whatever
+    the mask, so one set serves every job of a shape (CUDA graphs keep their addresses)."""
+
+    def __init__(self, total: int, device, with_noise: bool = True):
+        lib = _native.load()
+        n_words = int(lib.lp_known_words(total))
+        if n_words < 0:
+            raise ValueError(f"{total} elements: too many for the known-operand layout")
+        self.total = total
+        self.words = torch.empty(n_words, dtype=torch.int32, device=device)
+        self.y = torch.empty(total + 4, dtype=torch.float32, device=device)
+        self.noise = torch.empty(total + 4, dtype=torch.float32, device=device) if with_noise else None
+        self.struct = _native.Known(self.words.data_ptr(), self.y.data_ptr(),
+                                    self.noise.data_ptr() if with_noise else None)
+
+
+def pack_known(pm: PackedMask, dims, y: torch.Tensor, noise: Optional[torch.Tensor] = None,
+               out: Optional[KnownOperands] = None) -> KnownOperands:
+    """Fill (or allocate) the known-operand layout of mask `pm` and the dense fp32 y / noise (lp_pack_known, three
+    small launches on the current stream).  The dense operands stay in use by every kernel that reads them dense."""
+    total = y.numel()
+    if out is None or out.total != total or (noise is not None and out.noise is None):
+        out = KnownOperands(total, y.device, noise is not None)
+    lib = _native.load()
+    rc = lib.lp_pack_known(_P(pm.data.data_ptr()), C.byref(dims), _P(y.data_ptr()),
+                           _P(noise.data_ptr()) if noise is not None else None, _P(out.words.data_ptr()),
+                           _P(out.y.data_ptr()), _P(out.noise.data_ptr()) if noise is not None else None,
+                           _P(_stream_ptr(y.device)))
+    _native.check(rc, "lp_pack_known")
+    return out
 
 
 def pack_mask(latent_mask: torch.Tensor, like: torch.Tensor) -> PackedMask:
@@ -498,6 +537,8 @@ class LanPaint:
         stream = _P(_stream_ptr(dev))
         F = _native
         noise_arg = nz
+        # the known-operand layout, when the owner of y / nz / pm built it for exactly these operands
+        kn = getattr(pm, "known", None)
         if call_scaling:  # opaque noise_scaling: call it like the reference does (lanpaint.py:88)
             sampling = self.inner_model.inner_model.model_sampling
             noise_arg = _f32c(sampling.noise_scaling(self.add_none_dims(sigma_dev), nz, y))
@@ -531,9 +572,14 @@ class LanPaint:
                 r = plan.rng_struct(2 if (has_next and not merge) else 1, rng_state)
                 ev = self._event_pair(flags) if self.kernel_timer is not None else None
                 # heads of any dtype; with a CfgPair both CFG combines happen inside the kernel
-                rc = lib.lp_substep(_P(xm.data_ptr()), C.byref(hd), _P(y.data_ptr()), _P(pm.data.data_ptr()),
-                                    _P(cbuf.data_ptr()), None, None, _P(tab.data_ptr()), C.byref(dims), C.byref(r),
-                                    flags, stream)
+                if kn is not None:
+                    rc = lib.lp_substep_known(_P(xm.data_ptr()), C.byref(hd), _P(y.data_ptr()), _P(pm.data.data_ptr()),
+                                              C.byref(kn.struct), _P(cbuf.data_ptr()), None, None, _P(tab.data_ptr()),
+                                              C.byref(dims), C.byref(r), flags, stream)
+                else:
+                    rc = lib.lp_substep(_P(xm.data_ptr()), C.byref(hd), _P(y.data_ptr()), _P(pm.data.data_ptr()),
+                                        _P(cbuf.data_ptr()), None, None, _P(tab.data_ptr()), C.byref(dims), C.byref(r),
+                                        flags, stream)
                 if ev is not None:
                     ev[1].record()
                 _native.check(rc, "lp_substep")
@@ -595,10 +641,17 @@ class LanPaint:
             mo, _ = self.unpack_model_output(out_heads)
             hd, keep = _heads(mo, None, xm)
         fused_next = next_table is not None and euler_coef is not None
-        rc = lib.lp_boundary(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()) if fused_next else None,
-                             _P(pm.data.data_ptr()), _P(xm.data_ptr()) if euler_coef is not None else None,
-                             _P(_ptr(out)), C.c_float(euler_coef or 0.0),
-                             _P(next_table.data_ptr()) if fused_next else None, C.byref(dims), stream)
+        if kn is not None and (kn.noise is not None or not fused_next):
+            rc = lib.lp_boundary_known(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()) if fused_next else None,
+                                       _P(pm.data.data_ptr()), C.byref(kn.struct),
+                                       _P(xm.data_ptr()) if euler_coef is not None else None, _P(_ptr(out)),
+                                       C.c_float(euler_coef or 0.0), _P(next_table.data_ptr()) if fused_next else None,
+                                       C.byref(dims), stream)
+        else:
+            rc = lib.lp_boundary(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()) if fused_next else None,
+                                 _P(pm.data.data_ptr()), _P(xm.data_ptr()) if euler_coef is not None else None,
+                                 _P(_ptr(out)), C.c_float(euler_coef or 0.0),
+                                 _P(next_table.data_ptr()) if fused_next else None, C.byref(dims), stream)
         _native.check(rc, "lp_boundary")
         self.launches += 1
         return done

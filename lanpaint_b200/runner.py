@@ -400,7 +400,7 @@ class GraphedJob:
     def load_inputs(self, latent_image: torch.Tensor, noise: torch.Tensor, mask, x_init=None):
         """Copies of the request's own inputs into the static buffers (H2D when they are host tensors)."""
         import numpy as np
-        from .engine import PackedMask, pack_mask
+        from .engine import PackedMask, pack_known, pack_mask
         self.y.copy_(latent_image, non_blocking=True)
         if noise is None:   # serving hosts that do not need ComfyUI's CPU noise image: draw it on the device
             self.noise.normal_()
@@ -417,6 +417,8 @@ class GraphedJob:
         B = self.shape[0]
         self._dims = _native.Dims(B, self.x.numel() // B, int(np.prod(self.shape[2:])), self.mask.row_stride,
                                   self.mask.channel_stride)
+        # y and the noise image at known positions only, for the kernels that stream them (same buffers every job)
+        self.mask.known = pack_known(self.mask, self._dims, self.y, self.noise, out=self.mask.known)
 
     def run(self, latent_image: torch.Tensor, noise: torch.Tensor, mask, x_out: Optional[torch.Tensor] = None,
             x_init: Optional[torch.Tensor] = None, callback=None, mode: Optional[str] = None, warm: bool = True):
@@ -522,7 +524,7 @@ class SamplerGraphJob:
 
     def _load(self, latent_image, noise, pm, x_init):
         import numpy as np
-        from .engine import PackedMask
+        from .engine import PackedMask, pack_known
         self.y.copy_(latent_image, non_blocking=True)
         self.noise.copy_(noise, non_blocking=True)
         self.x0.copy_(x_init, non_blocking=True)
@@ -534,6 +536,7 @@ class SamplerGraphJob:
         B = self.shape[0]
         self.dims = _native.Dims(B, self.x0.numel() // B, int(np.prod(self.shape[2:])), self.mask.row_stride,
                                  self.mask.channel_stride)
+        self.mask.known = pack_known(self.mask, self.dims, self.y, self.noise, out=self.mask.known)
 
     def _capture(self, model_k, extra_args, want_callbacks):
         eng = self.engine
