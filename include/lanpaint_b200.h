@@ -158,6 +158,14 @@ int64_t lp_selftest_index_math(int64_t samples);
  * mismatches into *mismatches_dev (a device uint64, zeroed by the call).  0 = the two are interchangeable. */
 int lp_selftest_box_muller(int64_t n, uint64_t seed, unsigned long long* mismatches_dev, lp_stream_t stream);
 
+/* Device self test of the LP_RNG_PHILOX Box-Muller (MUFU lg2 / sqrt / sin / cos) over all 2^32 values of one input
+ * word: the first word (sweep_second == 0) or the second, the other held at fixed_word.  *nonfinite_dev (a device
+ * uint64) receives the number of inputs with a non-finite output and *max_err_dev (a device double) the largest
+ * |fast - fp64 Box-Muller| over both outputs, the fp64 transform taken of the same fp32 u and v.  Both are zeroed by
+ * the call. */
+int lp_selftest_normal_fast(uint32_t fixed_word, int sweep_second, unsigned long long* nonfinite_dev,
+                            double* max_err_dev, lp_stream_t stream);
+
 /* ---- host: coefficient table ------------------------------------------- */
 /* Replaces LanPaint.prepare_step_size + the mask blend of A/D/dt + the
  * exp/expm1/where/sqrt of advance_time_overdamped (lanpaint.py:81,205-214,

@@ -22,7 +22,7 @@ SUBSTEP_FIRST, SUBSTEP_FUSE_NEXT, SUBSTEP_STORE_C, SUBSTEP_MERGE_NOISE = 1, 2, 4
 
 # every symbol include/lanpaint_b200.h declares (checked by tests/test_abi.py)
 SYMBOLS = (
-    "lp_abi_version", "lp_status_string", "lp_last_cuda_error", "lp_set_option", "lp_selftest_index_math", "lp_selftest_box_muller", "lp_build_coef_table", "lp_build_coef_table_dt",
+    "lp_abi_version", "lp_status_string", "lp_last_cuda_error", "lp_set_option", "lp_selftest_index_math", "lp_selftest_box_muller", "lp_selftest_normal_fast", "lp_build_coef_table", "lp_build_coef_table_dt",
     "lp_torch_randn_geometry", "lp_pack_mask_f32", "lp_prologue_f32", "lp_substep", "lp_substep_f32", "lp_substep_cfg_f32", "lp_advance_f32",
     "lp_boundary", "lp_synth_denoiser", "lp_known_words", "lp_pack_known", "lp_substep_known", "lp_boundary_known",
     "lp_epilogue_f32", "lp_epilogue_euler_f32", "lp_step_boundary_f32", "lp_epilogue_cfg_f32", "lp_stop_stats_f32", "lp_fill_normal_f32", "lp_synth_denoiser_f32", "lp_l2_persist_capacity", "lp_l2_persist_set", "lp_l2_persist_clear", "lp_l2_flush", "lp_torch_cpu_randn_f32",
@@ -89,6 +89,8 @@ def load() -> C.CDLL:
     lib.lp_selftest_index_math.argtypes = [i64]
     lib.lp_selftest_box_muller.restype = i32
     lib.lp_selftest_box_muller.argtypes = [i64, u64, p, p]
+    lib.lp_selftest_normal_fast.restype = i32
+    lib.lp_selftest_normal_fast.argtypes = [C.c_uint32, i32, p, p, p]
     lib.lp_build_coef_table.restype = i32
     lib.lp_build_coef_table.argtypes = [p, p, p, p, p, i64, C.POINTER(Hyper), p]
     lib.lp_build_coef_table_dt.restype = i32

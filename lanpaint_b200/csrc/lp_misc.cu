@@ -245,6 +245,41 @@ __global__ void __launch_bounds__(kBlock) selftest_box_muller_kernel(uint64_t n,
   if (mine) atomicAdd(bad, mine);
 }
 
+// box_muller_fast (the LP_RNG_PHILOX transform) over all 2^32 values of one input word, the other word fixed:
+// counts non-finite outputs and takes the largest |fast - fp64 Box-Muller of the same fp32 u and v|
+__global__ void __launch_bounds__(kBlock) selftest_normal_fast_kernel(uint32_t fixed, int sweep_second,
+                                                                      unsigned long long* nonfinite,
+                                                                      unsigned long long* max_err_bits) {
+  pdl_prologue();
+  const uint64_t gid = (uint64_t)blockIdx.x * kBlock + threadIdx.x;
+  const uint64_t stride = (uint64_t)gridDim.x * kBlock;
+  unsigned long long bad = 0;
+  double worst = 0.0;
+  for (uint64_t w = gid; w < (1ull << 32); w += stride) {
+    const uint32_t a = sweep_second ? fixed : (uint32_t)w, b = sweep_second ? (uint32_t)w : fixed;
+    const float2 r = box_muller_fast(a, b);
+    if (!isfinite(r.x) || !isfinite(r.y)) {
+      ++bad;
+      continue;
+    }
+    // the fp32 u and v box_muller_fast starts from, then the transform in fp64
+    const float u = a * 2.3283064e-10f + (2.3283064e-10f / 2);
+    const float v = b * (2.3283064e-10f * 6.2831855f) + ((2.3283064e-10f * 6.2831855f) / 2);
+    const double s = sqrt(-2.0 * log((double)u));
+    double sn, cs;
+    sincos((double)v, &sn, &cs);
+    worst = fmax(worst, fmax(fabs((double)r.x - s * sn), fabs((double)r.y - s * cs)));
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    bad += __shfl_xor_sync(0xffffffffu, bad, o);
+    worst = fmax(worst, __shfl_xor_sync(0xffffffffu, worst, o));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    if (bad) atomicAdd(nonfinite, bad);
+    atomicMax(max_err_bits, (unsigned long long)__double_as_longlong(worst));  // worst >= 0: bits order like values
+  }
+}
+
 template <int N, typename H>
 __global__ void __launch_bounds__(kBlock) synth_denoiser_kernel(const float* __restrict__ x, H* h0, H* h1, uint32_t n,
                                                                 float a0, float b0, float c0, float a1, float c1) {
@@ -350,6 +385,19 @@ extern "C" int lp_selftest_box_muller(int64_t n, uint64_t seed, unsigned long lo
   if (n == 0) return LP_OK;
   const unsigned grid = (unsigned)device_info(current_device()).sms * 8u;
   launch_kernel(selftest_box_muller_kernel, dim3(grid), s, (uint64_t)n, seed, mismatches_dev);
+  return check_launch();
+}
+
+extern "C" int lp_selftest_normal_fast(uint32_t fixed_word, int sweep_second, unsigned long long* nonfinite_dev,
+                                       double* max_err_dev, lp_stream_t stream) {
+  if (!nonfinite_dev || !max_err_dev) return LP_ERR_INVALID;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (cudaMemsetAsync(nonfinite_dev, 0, sizeof(unsigned long long), s) != cudaSuccess ||
+      cudaMemsetAsync(max_err_dev, 0, sizeof(double), s) != cudaSuccess)
+    return (check_launch(), LP_ERR_CUDA);
+  const unsigned grid = (unsigned)device_info(current_device()).sms * 8u;
+  launch_kernel(selftest_normal_fast_kernel, dim3(grid), s, fixed_word, sweep_second, nonfinite_dev,
+                reinterpret_cast<unsigned long long*>(max_err_dev));
   return check_launch();
 }
 

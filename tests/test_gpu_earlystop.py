@@ -60,6 +60,51 @@ def test_early_stop_matches_reference_trace(name, cuda_device):
     assert max_rel(x, torch.from_numpy(g["x_new"])) <= 2e-5
 
 
+def test_torch_stream_early_stop_equals_its_tape(cuda_device):
+    """The early-stop loop under the default torch stream (lp_advance_f32 -> advance_torch_kernel, lp_substep with
+    the x0e side output) against the same loop fed a NoiseTape of the torch.randn draws the reference makes from the
+    same seed, in its order (1 draw for sub-step 0, then 2 per sub-step).  The tape path is pinned to the
+    reference's own stopper by test_early_stop_matches_reference_trace; the stop (min_steps 4 with a threshold
+    every distance passes) fires mid-loop whatever the noise.  Same draws, same per-element arithmetic: the stop
+    trace, the outputs and the generator's final offset must be identical."""
+    from lanpaint_b200.engine import LanPaint, NoiseTape
+    g = load_golden("aux_es_min_steps_legacy")
+    meta = g["meta"]
+    dev = cuda_device
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    y, noise, mask, sigma = t(g["y"]), t(g["noise"]), t(g["mask_full"]), t(g["sigma"])
+    times = (t(g["ve"]), t(g["abt"]), t(g["flow_t"]))
+    gen = torch.cuda.default_generators[dev.index or 0]
+    n = meta["n_steps"]
+
+    def run(rng):
+        model = make_model("two_heads", False)
+        eng = LanPaint(model, NSteps=n, Friction=15.0, Lambda=5.0, Beta=1.0, StepSize=0.2, MinStepFrac=1.0,
+                       EarlyStopThreshold=meta["ctor_threshold"], EarlyStopPatience=meta["ctor_patience"], rng=rng)
+        trace = []
+        mo = {"lanpaint_semantic_trace": trace, "lanpaint_semantic_stop": dict(meta["stop"])}
+        x = t(g["x"])
+        out = eng(x, y, noise, sigma, mask, times, mo, 0, n_steps=n)
+        return out, x, trace, model.calls
+
+    torch.manual_seed(1234)
+    off0 = gen.get_offset()
+    draws = [torch.randn_like(y) for _ in range(2 * n - 1)]     # every draw the reference could make, in its order
+    inc = (gen.get_offset() - off0) // (2 * n - 1)
+    tape = NoiseTape(draws)
+    want = run(tape)
+    assert 0 < tape.pos < 2 * n - 1, tape.pos                     # stopped mid-loop
+    torch.manual_seed(1234)
+    got = run("torch")
+    assert len(got[2]) == len(want[2]) and got[3] == want[3]
+    for a, b in zip(got[2], want[2]):
+        for k in ("inner_step", "patience_counter", "patience_eff", "stopped", "dist", "dist_inpaint", "dist_ring",
+                  "dist_drift", "threshold", "threshold_eff", "abt"):
+            assert a[k] == b[k], (k, a, b)
+    assert torch.equal(got[0], want[0]) and torch.equal(got[1], want[1])
+    assert gen.get_offset() == off0 + tape.pos * inc             # advanced by exactly the draws consumed
+
+
 def test_stats_kernel_matches_torch(cuda_device):
     import ctypes as C
     from lanpaint_b200 import _native
