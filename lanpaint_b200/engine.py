@@ -909,6 +909,8 @@ class LanPaint:
         rep_y = [float(f32(1.0) - f32(s_v))] * lines + [float(f32(1.0) - f32(s_au))] * lines
         table_np = build_table([abt_v] * lines + [abt_au] * lines, [ve_v] * lines + [ve_au] * lines, hyper,
                                rep_n, rep_y, [1.0] * lines + [c_au] * lines)
+        if split == 0:   # an all-audio pack: row_split 0 means "no split", so every line reads the audio rows alone
+            table_np = table_np[lines:]
 
         xm = x if (x.dtype == torch.float32 and x.is_contiguous()) else _f32c(x)
         y = _f32c(self.latent_image.to(dev))
@@ -932,7 +934,8 @@ class LanPaint:
         dims = _native.Dims(lines, n_last, n_last, n_last, 0, split)
         tab = torch.from_numpy(table_np).to(dev)
         t_model = t_model_src.reshape(-1).to(dev)
-        active = n_steps if mean_half_dt([abt_v, abt_au], hyper) > 0.0 else 0
+        present = ([abt_v] if split > 0 else []) + ([abt_au] if split < n_last else [])   # the schedules in use
+        active = n_steps if mean_half_dt(present, hyper) > 0.0 else 0
         plan = _DrawPlan(rng, xm, active)
         out = torch.empty_like(xm)
         cbuf = torch.empty_like(xm)

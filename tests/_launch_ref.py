@@ -7,6 +7,12 @@ ou_advance, the masked score), in the table form the kernels use:
 and it reads every per-element coefficient from the same fp32 table row the kernel reads (LP_T_* / LP_C_*), so it
 checks the kernels, not lp_build_coef_table (tests/test_table_properties.py covers the table).
 
+Table rows: by default element b of the leading axis reads row b (the tensors are shaped so that the leading axis is
+lp_dims.n_rows).  With a row split (the audio-video flat pack), pass rows = split_rows(shape, row_split): the
+per-element row index, n_rows + b at positions >= row_split within row b.  The audio target correction LP_T_CORR
+is restated as the kernel and the oracle's masked_score apply it: x0' = x + corr (x0 - x) on the model-space x,
+after the CFG combine, on both heads.
+
 Each function returns the fp64 value and, for the fp32 outputs, the magnitude chain: the same expression evaluated
 on the absolute values of every operand and coefficient with subtractions turned into additions.  A kernel that
 evaluates the expression in fp32 with n roundings on the longest path is within n * 2^-24 * magnitude of the fp64
@@ -100,12 +106,24 @@ def torch_stream_normals(n: int, seed: int, offset: int, T: int) -> np.ndarray:
 # ---------------------------------------------------------------------------------------------------------------
 # per-element coefficients out of the fp32 table
 # ---------------------------------------------------------------------------------------------------------------
-def _row(tab: torch.Tensor, col: int, ndim: int) -> torch.Tensor:
+def split_rows(shape, row_split: int, device=None) -> torch.Tensor:
+    """The table row of every element of a launch with lp_dims.n_rows = shape[0], per_row = the rest of the shape and
+    lp_dims.row_split = row_split: b, or n_rows + b at positions r >= row_split of row b (row_split 0 = off)."""
+    n_rows, per_row = shape[0], int(np.prod(shape[1:]))
+    b = torch.arange(n_rows, device=device).view(-1, 1)
+    r = torch.arange(per_row, device=device).view(1, -1)
+    rows = b + (n_rows * (r >= row_split) if row_split else 0 * r)
+    return rows.reshape(shape)
+
+
+def _row(tab: torch.Tensor, col: int, ndim: int, rows=None) -> torch.Tensor:
+    if rows is not None:
+        return tab[:, col].double()[rows]
     return tab[:, col].double().view((-1,) + (1,) * (ndim - 1))
 
 
-def _cls(tab, known, col, ndim):
-    return torch.where(known, _row(tab, T_CLS1 + col, ndim), _row(tab, T_CLS0 + col, ndim))
+def _cls(tab, known, col, ndim, rows=None):
+    return torch.where(known, _row(tab, T_CLS1 + col, ndim, rows), _row(tab, T_CLS0 + col, ndim, rows))
 
 
 class _Val:
@@ -120,83 +138,89 @@ class _Mag:
     sub = staticmethod(lambda a, b: a + b)
 
 
-def _substep_expr(m, x, a, b, y, cp, xi1, xi2, tab, known, flags, cfg):
+def _substep_expr(m, x, a, b, y, cp, xi1, xi2, tab, known, flags, cfg, rows):
     """lp_substep of the header, in the arithmetic m: (x', C', x_t + score)."""
     nd = x.ndim
     A = m.abs
+    row = lambda col: A(_row(tab, col, nd, rows))
+    cls = lambda col: A(_cls(tab, known, col, nd, rows))
     first, nxt, merge = bool(flags & FIRST), bool(flags & FUSE_NEXT), bool(flags & MERGE_NOISE)
     if cfg is not None:   # x0 = uncond + (cond - uncond) * cfg ; x0_BIG = uncond + (cond - uncond) * cfg_big
         d = m.sub(a, b)
         a, b = b + d * A(cfg[0]), b + d * A(cfg[1])
-    lam, opl = A(_row(tab, T_LAM, nd)), A(_row(tab, T_ONEPLAM, nd))
+    if bool(torch.any(tab[:, T_CORR] != 1)):   # audio rows: x0 = x + corr (x0 - x) on both heads, model-space x
+        corr = _row(tab, T_CORR, nd, rows)
+        on = corr != 1
+        a = torch.where(on, x + A(corr) * m.sub(a, x), a)
+        b = torch.where(on, x + A(corr) * m.sub(b, x), b)
+    lam, opl = row(T_LAM), row(T_ONEPLAM)
     tgt = torch.where(known, m.sub(opl * y, lam * b), a)                      # x_t + score (masked score)
-    xt = x * A(_row(tab, T_INVS, nd))                                          # model space -> x_t
-    cn = A(_row(tab, T_CTGT, nd)) * tgt + A(_cls(tab, known, C_G, nd)) * xt    # Coef_C, table form
+    xt = x * row(T_INVS)                                                       # model space -> x_t
+    cn = row(T_CTGT) * tgt + cls(C_G) * xt                                     # Coef_C, table form
     full = first
-    e1, k1, s1 = (A(_cls(tab, known, c, nd)) for c in ((C_EF, C_KF, C_SF) if full else (C_EH, C_KH, C_SH)))
-    e2, k2, s2 = (A(_cls(tab, known, c, nd)) for c in (C_EH, C_KH, C_SH))
+    e1, k1, s1 = (cls(c) for c in ((C_EF, C_KF, C_SF) if full else (C_EH, C_KH, C_SH)))
+    e2, k2, s2 = (cls(c) for c in (C_EH, C_KH, C_SH))
     if not first:                                                              # x += (Cn - C) dt, advance with old C
-        xt = xt + m.sub(cn, cp) * A(_cls(tab, known, C_DT, nd))
+        xt = xt + m.sub(cn, cp) * cls(C_DT)
     c_adv = cn if first else cp
     if merge:   # both kicks as one Gaussian of the summed variance, after the second advance
-        sm = A(torch.where(known, _row(tab, (T_SDMF if first else T_SDM) + 1, nd), _row(tab, T_SDMF if first else T_SDM, nd)))
+        col = T_SDMF if first else T_SDM
+        sm = torch.where(known, row(col + 1), row(col))
         xt = e1 * xt + k1 * c_adv
         xt = e2 * xt + k2 * cn + sm * xi1
     else:
         xt = e1 * xt + k1 * c_adv + s1 * xi1                                   # ou_advance
         if nxt:
             xt = e2 * xt + k2 * cn + s2 * xi2
-    return xt * A(_row(tab, T_S, nd)), cn, tgt
+    return xt * row(T_S), cn, tgt
 
 
 def _d(t):
     return None if t is None else (t.double() if torch.is_tensor(t) else torch.as_tensor(t, dtype=torch.float64))
 
 
-def substep(x, a, b, y, known, cprev, tab, xi1, xi2, flags, cfg=None, noise_err=0.0):
+def substep(x, a, b, y, known, cprev, tab, xi1, xi2, flags, cfg=None, noise_err=0.0, rows=None):
     """One lp_substep launch.  a, b: the heads as the kernel reads them (widened here; b None = aliased);
     cfg = (cfg, cfg_big) when a, b are cond / uncond.  xi1 / xi2: the draws (fp64 or fp32 tensors).
-    noise_err: largest error of each kernel draw against xi (the philox transform's).
+    noise_err: largest error of each kernel draw against xi (the philox transform's).  rows: see split_rows.
     Returns dict(x, c, x0e) of (value, magnitude) pairs and x_slack, the absolute error noise_err can cause in x."""
-    if torch.any(tab[:, T_CORR] != 1):
-        raise NotImplementedError("rows with the audio target correction")
     b = a if b is None else b
     z = torch.zeros((), dtype=torch.float64, device=x.device)
     cp = z if cprev is None or flags & FIRST else _d(cprev)
     xi2 = z if xi2 is None else _d(xi2)
     ops = [_d(x), _d(a), _d(b), _d(y), cp, _d(xi1), xi2]
-    val = _substep_expr(_Val, *ops, tab, known, flags, cfg)
-    mag = _substep_expr(_Mag, *[o.abs() for o in ops], tab, known, flags, cfg)
+    val = _substep_expr(_Val, *ops, tab, known, flags, cfg, rows)
+    mag = _substep_expr(_Mag, *[o.abs() for o in ops], tab, known, flags, cfg, rows)
     slack = 0.0
     if noise_err:   # the chain is linear in the draws: its magnitude with every other operand 0
         zx = torch.zeros_like(ops[0])
         ne = torch.full_like(zx, noise_err)
-        slack = _substep_expr(_Mag, zx, zx, zx, zx, zx, ne, ne, tab, known, flags, cfg)[0]
+        slack = _substep_expr(_Mag, zx, zx, zx, zx, zx, ne, ne, tab, known, flags, cfg, rows)[0]
     return {"x": (val[0], mag[0]), "c": (val[1], mag[1]), "x0e": (val[2], mag[2]), "x_slack": slack}
 
 
-def advance(x, c, known, tab, xi, half):
+def advance(x, c, known, tab, xi, half, rows=None):
     """lp_advance_f32: x_t = x / S ; x_t = e x_t + k C + sd xi ; x = x_t S  (ou_advance over dt or dt/2)."""
     def expr(m, x, c, xi):
         A, nd = m.abs, x.ndim
         cols = (C_EH, C_KH, C_SH) if half else (C_EF, C_KF, C_SF)
-        e, k, sd = (A(_cls(tab, known, col, nd)) for col in cols)
-        xt = x * A(_row(tab, T_INVS, nd))
-        return (e * xt + k * c + sd * xi) * A(_row(tab, T_S, nd))
+        e, k, sd = (A(_cls(tab, known, col, nd, rows)) for col in cols)
+        xt = x * A(_row(tab, T_INVS, nd, rows))
+        return (e * xt + k * c + sd * xi) * A(_row(tab, T_S, nd, rows))
     ops = [_d(x), _d(c), _d(xi)]
     return expr(_Val, *ops), expr(_Mag, *[o.abs() for o in ops])
 
 
-def prologue(x, y, noise, known, tab):
+def prologue(x, y, noise, known, tab, rows=None):
     """lp_prologue_f32: x_model = known ? rep_noise * noise + rep_y * y : x."""
     nd = x.ndim
-    rn, ry = _row(tab, T_REPN, nd), _row(tab, T_REPY, nd)
+    rn, ry = _row(tab, T_REPN, nd, rows), _row(tab, T_REPY, nd, rows)
     val = torch.where(known, rn * _d(noise) + ry * _d(y), _d(x))
     mag = torch.where(known, rn.abs() * _d(noise).abs() + ry.abs() * _d(y).abs(), _d(x).abs())
     return val, mag
 
 
-def boundary(a, b, y, noise, known, x, coef, next_tab, cfg=None):
+def boundary(a, b, y, noise, known, x, coef, next_tab, cfg=None, rows=None):
     """lp_boundary: d = combine ? b + (a - b) cfg : a ; out = known ? y : d ; x = x + (x - out) coef (x given) ;
     x = known ? rep_noise * noise + rep_y * y : x (next_tab given).  -> dict(out, x) of (value, magnitude)."""
     def expr(m, a, b, y, noise, x):
@@ -208,7 +232,8 @@ def boundary(a, b, y, noise, known, x, coef, next_tab, cfg=None):
         x = x + m.sub(x, out) * A(coef)
         if next_tab is not None:
             nd = x.ndim
-            x = torch.where(known, A(_row(next_tab, T_REPN, nd)) * noise + A(_row(next_tab, T_REPY, nd)) * y, x)
+            rn, ry = A(_row(next_tab, T_REPN, nd, rows)), A(_row(next_tab, T_REPY, nd, rows))
+            x = torch.where(known, rn * noise + ry * y, x)
         return out, x
     z = torch.zeros((), dtype=torch.float64, device=y.device)
     ops = [_d(a), z if b is None else _d(b), _d(y), z if noise is None else _d(noise), _d(x)]
@@ -217,9 +242,9 @@ def boundary(a, b, y, noise, known, x, coef, next_tab, cfg=None):
     return {"out": (val[0], mag[0]), "x": (val[1], mag[1])}
 
 
-def stop_stats(a, b, known, ring, tab):
+def stop_stats(a, b, known, ring, tab, rows=None):
     """lp_stop_stats_f32: (sum over free elements, sum over ring elements) of (inv_S (a - b))^2, fp64."""
-    d2 = ((_d(a) - _d(b)) * (_row(tab, T_INVS, a.ndim) if tab is not None else 1.0)) ** 2
+    d2 = ((_d(a) - _d(b)) * (_row(tab, T_INVS, a.ndim, rows) if tab is not None else 1.0)) ** 2
     s_in = float(torch.where(known, torch.zeros_like(d2), d2).sum())
     s_ring = float(torch.where(ring, d2, torch.zeros_like(d2)).sum()) if ring is not None else 0.0
     return s_in, s_ring

@@ -258,6 +258,53 @@ def dump_earlystop():
                             abt=times.abt.numpy(), flow_t=times.flow_t.numpy(),
                             tape=np.stack([d.numpy() for d in tape.recorded]), out=out.numpy(), x_new=x_ref.numpy(),
                             meta=np.array(json.dumps(meta)))
+    dump_earlystop_av()
+
+
+# the early stopper on AV flat packs [1, C, N] (flow): the last N - video_n positions on the audio schedule, with
+# and without the target correction; the stopper's threshold scales with the blended abt (lanpaint.py:104-111)
+EARLYSTOP_AV_CASES = [
+    dict(name="aux_es_av_midway", shape=(1, 4, 48), video_n=32, sigma=0.5, sigma_a=0.3, corr=0.8,
+         stop={"threshold": 0.3, "patience": 2}, n=10),
+    dict(name="aux_es_av_nocorr", shape=(1, 1, 96), video_n=61, sigma=0.7, sigma_a=0.45, corr=None,
+         stop={"threshold": 0.3, "patience": 1}, n=10),
+]
+
+
+def dump_earlystop_av():
+    torch.set_num_threads(1)
+    for c in EARLYSTOP_AV_CASES:
+        g = torch.Generator().manual_seed(13)
+        shape = c["shape"]
+        x, y, noise = (torch.randn(shape, generator=g) for _ in range(3))
+        mask = (torch.rand(shape, generator=g) < 0.5).float()
+        sigma, sig_a = torch.tensor([c["sigma"]]), torch.tensor([c["sigma_a"]])
+        times, times_a = O.times_from_sigma(sigma, True), O.times_from_sigma(sig_a, True)
+        ai = torch.zeros((1, 1, shape[-1]))
+        ai[..., c["video_n"]:] = 1.0
+        corr = None if c["corr"] is None else (1.0 - ai) + c["corr"] * ai
+        tape = O.NoiseTape(generator=torch.Generator().manual_seed(4))
+        model = make_model("two_heads", True)
+        eng = RefEngine(model, NSteps=c["n"], Friction=15.0, Lambda=5.0, Beta=1.0, StepSize=0.2, IS_FLOW=True,
+                        MinStepFrac=1.0)
+        trace = []
+        mo = {"lanpaint_semantic_trace": trace, "bench_case_id": c["name"], "bench_outer_step": 3,
+              "bench_timestep": 0.5, "lanpaint_semantic_stop": dict(c["stop"])}
+        x_ref = x.clone()
+        with mock.patch.object(torch, "randn_like", tape):
+            out = eng(x_ref, y, noise, sigma, mask, tuple(times), model_options=mo, seed=0, n_steps=c["n"],
+                      current_times_audio=tuple(times_a), audio_indicator=ai, audio_correction=corr)
+        meta = dict(name=c["name"], n_steps=c["n"], video_n=c["video_n"], corr=c["corr"], stop=c["stop"], trace=trace,
+                    model_calls=model.calls, n_draws=len(tape.recorded))
+        print(f"{c['name']:28s} sub-steps run {len(trace):2d}/{c['n']} model calls {model.calls:2d} "
+              f"dists {[round(t['dist'], 4) for t in trace]}")
+        assert 1 < len(trace) < c["n"], "the case must stop midway"
+        np.savez_compressed(os.path.join(HERE, c["name"] + ".npz"), x=x.numpy(), y=y.numpy(), noise=noise.numpy(),
+                            sigma=sigma.numpy(), mask=mask.numpy().astype(np.uint8), ve=times.ve_sigma.numpy(),
+                            abt=times.abt.numpy(), flow_t=times.flow_t.numpy(), ve_a=times_a.ve_sigma.numpy(),
+                            abt_a=times_a.abt.numpy(), flow_a=times_a.flow_t.numpy(),
+                            tape=np.stack([d.numpy() for d in tape.recorded]), out=out.numpy(), x_new=x_ref.numpy(),
+                            meta=np.array(json.dumps(meta)))
 
 
 

@@ -12,7 +12,9 @@ from _support import make_model, max_rel
 
 pytestmark = pytest.mark.gpu
 
-ES_CASES = sorted(os.path.splitext(os.path.basename(p))[0] for p in glob.glob(os.path.join(GOLDEN_DIR, "aux_es_*.npz")))
+ES_ALL = sorted(os.path.splitext(os.path.basename(p))[0] for p in glob.glob(os.path.join(GOLDEN_DIR, "aux_es_*.npz")))
+ES_CASES = [n for n in ES_ALL if not n.startswith("aux_es_av_")]
+ES_AV_CASES = [n for n in ES_ALL if n.startswith("aux_es_av_")]
 
 
 def _custom_distance(prev, cur, ctx):
@@ -50,6 +52,46 @@ def test_early_stop_matches_reference_trace(name, cuda_device):
     out = eng(x, y, noise, sigma, mask, times, mo, 0, n_steps=meta["n_steps"])
     want = meta["trace"]
     assert len(trace) == len(want), (len(trace), len(want))          # stopped after the same sub-step
+    assert model.calls == meta["model_calls"] and tape.pos == meta["n_draws"]
+    for got, ref in zip(trace, want):
+        for k in ("inner_step", "patience_counter", "patience_eff", "custom_dist", "stopped", "case_id", "outer_step"):
+            assert got[k] == ref[k], (k, got, ref)
+        for k in ("dist", "dist_inpaint", "dist_ring", "dist_drift", "threshold", "threshold_eff", "abt"):
+            assert _close(got[k], ref[k]), (k, got[k], ref[k])
+    assert max_rel(out, torch.from_numpy(g["out"])) <= 2e-5
+    assert max_rel(x, torch.from_numpy(g["x_new"])) <= 2e-5
+
+
+@pytest.mark.parametrize("name", ES_AV_CASES)
+def test_early_stop_on_av_pack_matches_reference_trace(name, cuda_device):
+    """The stopper on an AV flat pack (audio suffix on its own schedule, with and without the target correction):
+    the reference stops midway, and the engine must stop after the same sub-step with the same distances, draws
+    and outputs."""
+    from lanpaint_b200.engine import LanPaint, NoiseTape
+    assert len(ES_AV_CASES) >= 2
+    g = load_golden(name)
+    meta = g["meta"]
+    dev = cuda_device
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    x, y, noise, mask = t(g["x"]), t(g["y"]), t(g["noise"]), t(g["mask_full"])
+    sigma = t(g["sigma"])
+    times = (t(g["ve"]), t(g["abt"]), t(g["flow_t"]))
+    times_a = (t(g["ve_a"]), t(g["abt_a"]), t(g["flow_a"]))
+    ai = torch.zeros((1, 1, x.shape[-1]), device=dev)
+    ai[..., meta["video_n"]:] = 1.0
+    corr = None if meta["corr"] is None else (1.0 - ai) + meta["corr"] * ai
+    tape = NoiseTape([t(d) for d in g["tape"]])
+    model = make_model("two_heads", True)
+    eng = LanPaint(model, NSteps=meta["n_steps"], Friction=15.0, Lambda=5.0, Beta=1.0, StepSize=0.2, IS_FLOW=True,
+                   MinStepFrac=1.0, rng=tape)
+    trace = []
+    mo = {"lanpaint_semantic_trace": trace, "bench_case_id": name, "bench_outer_step": 3, "bench_timestep": 0.5,
+          "lanpaint_semantic_stop": dict(meta["stop"])}
+    out = eng(x, y, noise, sigma, mask, times, mo, 0, n_steps=meta["n_steps"], current_times_audio=times_a,
+              audio_indicator=ai, audio_correction=corr)
+    want = meta["trace"]
+    assert 1 < len(want) < meta["n_steps"]
+    assert len(trace) == len(want), (len(trace), len(want))
     assert model.calls == meta["model_calls"] and tape.pos == meta["n_draws"]
     for got, ref in zip(trace, want):
         for k in ("inner_step", "patience_counter", "patience_eff", "custom_dist", "stopped", "case_id", "outer_step"):

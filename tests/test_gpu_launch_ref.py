@@ -26,7 +26,15 @@ The matrix is representative crossings, not a cross product:
   * the boundary sweep covers vec4 / scalar x dense / packed x the three dtypes, the TMA boundary kernel with and
     without combine and next, out-only launches and a zero Euler coefficient (replace step only);
   * prologue, advance (all three streams, one torch launch with several calls per subsequence and the state
-    block) and the early-stop statistics with the inv_S table and a full-shape ring at 8.4 M elements.
+    block) and the early-stop statistics with the inv_S table and a full-shape ring at 8.4 M elements;
+  * the audio-video flat pack (lp_dims.row_split, engine._av_call): every launch kind on every family a split can
+    reach (LDG vec4 / scalar on tape and philox with merge, torch vec4 and scalar), the boundary dense and packed,
+    prologue, advance on all three streams and the statistics, over 2 * lines distinct table rows whose audio rows
+    carry corrections != 1; one 4 Mi-element line split in the middle with TMA otherwise enabled, 16 lines split at
+    3/4, splits not a multiple of 4, an odd n_last, split == n_last and split == 4.  No TMA kernel may run under a
+    split (they find the row without it);
+  * the audio correction without a split on the TMA sub-step kernels, the only way to reach the corr code of the
+    torch TMA kernel's lane pairs.
 Coefficient tables mix VE rows sigma in {0.0292, 0.3, 1, 14.6, 80} and flow rows t in {0.02, 0.5, 0.98, 1}, with
 MinStepFrac 0, Lambda 0.1 or 12 and Beta 1.5 (distinct dt per mask class), or come from lp_build_coef_table_dt."""
 import collections
@@ -51,6 +59,7 @@ LP_DT = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 TMA_MIN = 1 << 18
 
 SEEN = collections.Counter()          # canonical kernel name -> launches
+SEEN_SPLIT = collections.Counter()    # the same, launches of cases with a row split
 WORST = collections.defaultdict(float)  # kernel family -> largest |got - want| / (2^-24 magnitude)
 RAN = set()
 
@@ -91,10 +100,11 @@ def rerun_on_lost_record(test):
     return wrapper
 
 
-def launched(fn):
+def launched(fn, split=None):
     """Run fn() (one library call returning its status) under torch.profiler -> set of canonical lp:: kernel names.
     The library call sits a few milliseconds inside the profiled window: the profiler keeps only device records whose
-    timestamps fall inside the window, and a launch of a few microseconds at its very edge can be dropped."""
+    timestamps fall inside the window, and a launch of a few microseconds at its very edge can be dropped.
+    split: the launch's row split (None: none), to record the kernels of split launches apart."""
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         time.sleep(0.005)
@@ -106,6 +116,8 @@ def launched(fn):
     got = {canon(n) for n in names}
     for n in got:
         SEEN[n] += 1
+        if split is not None:
+            SEEN_SPLIT[n] += 1
     return got
 
 
@@ -202,10 +214,29 @@ def offset_copy(t, nbytes):
     return v
 
 
-def dims_of(shape, rs, cs):
+def dims_of(shape, rs, cs, split=None):
     from lanpaint_b200 import _native
     sp = int(np.prod(shape[2:]))
-    return _native.Dims(shape[0], shape[1] * sp, sp, rs, cs, 0)
+    return _native.Dims(shape[0], shape[1] * sp, sp, rs, cs, split or 0)
+
+
+AV_CORR = (0.625, 1.3, 0.8)
+
+
+def case_table(c, shape, dev):
+    """-> (table, per-element rows or None).  A case with a "split" is an audio-video flat pack (one line per row,
+    shape (lines, 1, n_last)): 2 * lines distinct rows, the audio rows lines.. carrying the corrections AV_CORR in
+    turn, and every element reads the row split_rows gives it.  A case with "corr" (no split) sets the correction of
+    row b to corr[b % len(corr)]."""
+    split = c.get("split")
+    lines = shape[0]
+    tab = make_table(lines * (2 if split is not None else 1), c["table"], c["seed"], dev)
+    if split is not None:
+        tab[lines:, R.T_CORR] = torch.tensor([AV_CORR[b % 3] for b in range(lines)], device=dev)
+        return tab, R.split_rows(shape, split, dev)
+    if c.get("corr"):
+        tab[:, R.T_CORR] = torch.tensor([c["corr"][b % len(c["corr"])] for b in range(lines)], device=dev)
+    return tab, None
 
 
 def torch_T(n):
@@ -284,10 +315,11 @@ def expect_substep(c, shape, rs, cs):
     # a 16-bit head needs 8-byte alignment for the vec4 kernels, every other operand 16 bytes; TMA wants 16 everywhere
     head_mis = mis[0] == "a" or (mis[0] == "b" and c["heads"] == "sep")
     head_ok = not head_mis or (c["dtype"] != torch.float32 and mis[1] % 8 == 0)
-    v4 = (per_row % 4 == 0 and sp % 4 == 0 and rs % 4 == 0 and cs % 4 == 0
+    split = c.get("split")
+    v4 = (per_row % 4 == 0 and sp % 4 == 0 and rs % 4 == 0 and cs % 4 == 0 and (split or 0) % 4 == 0
           and mis[0] not in ("x", "y", "c", "tape0", "tape1") and head_ok)
     tma = (c.get("tma", 1) != 0 and sp % 16 == 0 and rs % 16 == 0 and cs % 16 == 0 and not side
-           and total >= c.get("tma_min", TMA_MIN) and mis[0] is None)
+           and total >= c.get("tma_min", TMA_MIN) and mis[0] is None and not split)
     if c["rng"].startswith("torch"):
         T, _ = torch_T(total)
         calls = -(-total // (4 * T))
@@ -311,9 +343,9 @@ def run_substep(c, dev, eps_bm):
     total = int(np.prod(shape))
     gen = torch.Generator(device=dev).manual_seed(c["seed"])
     m8, known, rs, cs = make_mask(shape, c["mask"], gen, dev)
-    dims = dims_of(shape, rs, cs)
-    tab = make_table(shape[0], c["table"], c["seed"], dev)
-    S = tab[:, 1].view((-1,) + (1,) * (len(shape) - 1))
+    dims = dims_of(shape, rs, cs, c.get("split"))
+    tab, rows = case_table(c, shape, dev)
+    S = R._row(tab, R.T_S, len(shape), rows).float()
     x = (torch.randn(shape, device=dev, generator=gen) * S).contiguous()
     y = torch.randn(shape, device=dev, generator=gen)
     cprev = torch.randn(shape, device=dev, generator=gen) * 3
@@ -373,6 +405,8 @@ def run_substep(c, dev, eps_bm):
     hd = _native.Heads(a.data_ptr(), None if c["heads"] == "null" else b.data_ptr(), LP_DT[c["dtype"]],
                        1 if cfg else 0, cfg[0] if cfg else 0.0, cfg[1] if cfg else 0.0)
     want_name = expect_substep(c, shape, rs, cs)
+    if "family" in c:   # the case reaches the family it was written for
+        assert family(want_name) == c["family"], (c["id"], want_name)
     y_dense = y
     if c.get("packed"):
         kn, keep_k = pack_known(m8, dims, y, None, total)
@@ -393,8 +427,8 @@ def run_substep(c, dev, eps_bm):
                                   C.byref(r), flags, _stream())
     x_in = x.clone()
     want = R.substep(x_in, a, None if c["heads"] == "null" else b, y, known, cprev, tab, xi1, xi2, flags, cfg=cfg,
-                     noise_err=noise_err)
-    got = launched(call)
+                     noise_err=noise_err, rows=rows)
+    got = launched(call, c.get("split"))
     fam = family(want_name)
     _check(fam, f"{c['id']} x", x, want["x"], slack=want["x_slack"])
     if writes_c:
@@ -512,9 +546,94 @@ EDGE += [
     dict(id="misalign8-b-bf16-philox", shape=(5, 4, 120, 136), rng="philox", flags=3, dtype=BF16, heads="sep",
          mask="full", table="lam12", misalign=("b", 8)),
 ]
+# the audio target correction without a split: the only way to reach the corr code of the TMA kernels (the torch
+# one in its lane-pair form); rows alternate corrections and 1
+EDGE += [
+    dict(id="corr-tma-philox-merge", shape=(5, 4, 120, 136), rng="philox", flags=2 | 8, dtype=F32, heads="sep",
+         mask="rand", table="lam12", corr=(0.625, 1.3, 1.0, 0.8), family="substep_tma_kernel"),
+    dict(id="corr-tma-philox-first-bf16", shape=(5, 4, 120, 136), rng="philox", flags=1, dtype=BF16, heads="null",
+         mask="full", table="dt", corr=(1.3, 1.0, 0.625), family="substep_tma_kernel"),
+    dict(id="corr-torch-tma-dense", shape=(5, 4, 120, 136), rng="torch", flags=3, dtype=F32, heads="sep", mask="rand",
+         table="dt", corr=(0.625, 1.3, 1.0, 0.8), family="substep_torch_tma_kernel"),
+    dict(id="corr-torch-tma-packed", shape=(5, 4, 120, 136), rng="torch", flags=2, dtype=BF16, heads="null",
+         mask="full", table="lam12", packed=True, corr=(0.8, 1.0, 1.3), family="substep_torch_tma_kernel"),
+    dict(id="corr-torch-tma-packed-cfg", shape=(5, 4, 120, 136), rng="torch_state", flags=0 | 4, dtype=F32,
+         heads="sep", mask="rand", table="lam01", packed=True, cfg=(4.5, -0.5), corr=(1.3, 0.625),
+         family="substep_torch_tma_kernel"),
+]
 for _i, _c in enumerate(EDGE):
     _c.setdefault("seed", 500 + _i)
-SUBSTEP_CASES = _sweep() + EDGE
+
+
+# the audio-video flat pack (engine._av_call): shape (lines, 1, n_last), lp_dims (lines, n_last, n_last, n_last, 0,
+# split), one uint8 mask element per latent element, 2 * lines table rows (case_table).  tma_min is 0 everywhere, so
+# that on the vec4 shapes only the split keeps the TMA kernels away.
+def _av_sweep():
+    cases = []
+    dts = (torch.float32, torch.bfloat16, torch.float16)
+    heads = ("sep", "null", "same")
+    masks = ("rand", "full", "rand", "known", "rand", "free")
+    kinds = (3, 1, 1 | 4, 2, 0, 0 | 4)
+    fams = [("av_ldg4_tape", "tape", (4, 1, 4096), 3072), ("av_ldg1_tape", "tape", (3, 1, 2049), 1000),
+            ("av_ldg4_philox", "philox", (4, 1, 4096), 3072), ("av_ldg1_philox", "philox", (4, 1, 4096), 3071),
+            ("av_torchvec", "torch", (4, 1, 4096), 3072), ("av_torch_scalar", "torch", (3, 1, 2049), 1000)]
+    i = 0
+    for name, rng, shape, split in fams:
+        for flags in kinds + ((3 | 8, 2 | 8) if rng == "philox" else ()):
+            cases.append(dict(id=f"{name}-f{flags}", shape=shape, split=split, rng=rng, flags=flags, dtype=dts[i % 3],
+                              heads=heads[(i // 3) % 3], mask=masks[i % 6], table=TABLES[i % 3], seed=700 + i,
+                              tma_min=0))
+            i += 1
+    return cases
+
+
+BIG = 1 << 22
+AV_EDGE = [
+    # one line of 4 Mi elements split in the middle (the torch stream: four calls per subsequence)
+    dict(id="av-big-torch-packed", shape=(1, 1, BIG), split=BIG // 2, rng="torch", flags=2, dtype=F32, heads="sep",
+         mask="rand", table="lam12", packed=True),
+    dict(id="av-big-torch-first-bf16", shape=(1, 1, BIG), split=BIG // 2, rng="torch", flags=3, dtype=BF16,
+         heads="null", mask="rand", table="dt"),
+    dict(id="av-big-philox-merge", shape=(1, 1, BIG), split=BIG // 2, rng="philox", flags=2 | 8, dtype=F32,
+         heads="sep", mask="rand", table="lam01"),
+    dict(id="av-big-tape-f16", shape=(1, 1, BIG), split=BIG // 2, rng="tape", flags=1 | 4, dtype=F16, heads="sep",
+         mask="rand", table="lam12"),
+    # 16 lines split at 3/4
+    dict(id="av-16-torch-packed", shape=(16, 1, 40960), split=30720, rng="torch", flags=3, dtype=F32, heads="sep",
+         mask="rand", table="lam12", packed=True),
+    dict(id="av-16-philox-cfg", shape=(16, 1, 40960), split=30720, rng="philox", flags=2, dtype=F32, heads="sep",
+         mask="full", table="dt", cfg=(4.5, -0.5)),
+    dict(id="av-16-tape-aliased-bf16", shape=(16, 1, 40960), split=30720, rng="tape", flags=0 | 4, dtype=BF16,
+         heads="same", mask="rand", table="lam01"),
+    # a split that is not a multiple of 4 on an n_last that is: the scalar kernels
+    dict(id="av-split3071-torch", shape=(4, 1, 4096), split=3071, rng="torch", flags=2, dtype=F32, heads="sep",
+         mask="rand", table="lam12"),
+    dict(id="av-split3071-philox-merge-bf16", shape=(4, 1, 4096), split=3071, rng="philox", flags=3 | 8, dtype=BF16,
+         heads="sep", mask="rand", table="dt"),
+    # an odd n_last
+    dict(id="av-odd-torch-f16", shape=(3, 1, 2049), split=1000, rng="torch", flags=3, dtype=F16, heads="null",
+         mask="rand", table="lam12"),
+    dict(id="av-odd-philox-state", shape=(3, 1, 2049), split=1000, rng="philox_state", flags=2, dtype=F32, heads="sep",
+         mask="rand", table="lam01"),
+    # split == n_last: the audio rows are never read (and the split still keeps TMA away)
+    dict(id="av-split-nlast-torch-packed", shape=(4, 1, 4096), split=4096, rng="torch", flags=2, dtype=F32,
+         heads="sep", mask="rand", table="lam12", packed=True),
+    dict(id="av-split-nlast-philox", shape=(4, 1, 4096), split=4096, rng="philox", flags=3, dtype=F32, heads="sep",
+         mask="rand", table="dt"),
+    # split == 4
+    dict(id="av-split4-torch-state", shape=(4, 1, 4096), split=4, rng="torch_state", flags=3, dtype=F32, heads="sep",
+         mask="rand", table="dt"),
+    dict(id="av-split4-tape-bf16", shape=(4, 1, 4096), split=4, rng="tape", flags=1, dtype=BF16, heads="sep",
+         mask="full", table="lam12"),
+    # the torch scalar kernel with two curand_normal4 calls per subsequence
+    dict(id="av-odd-torch-calls", shape=(1, 1, 1_200_001), split=600_001, rng="torch", flags=2, dtype=F32, heads="sep",
+         mask="rand", table="lam12"),
+]
+for _i, _c in enumerate(AV_EDGE):
+    _c.setdefault("seed", 800 + _i)
+    _c.setdefault("tma_min", 0)
+AV_CASES = _av_sweep() + AV_EDGE
+SUBSTEP_CASES = _sweep() + EDGE + AV_CASES
 
 
 @pytest.fixture
@@ -565,6 +684,22 @@ def _boundary_sweep():
         dict(id="b-misalign-noise", shape=(1, 4, 128, 128), dtype=F32, combine=None, next=True, out=True, euler=True,
              misalign="noise", mask="rand", table="lam12"),
     ]
+    # audio-video flat packs: the next table's rows follow the split; tma_boundary 1, so only the split keeps the
+    # TMA boundary kernel away from the vec4 ones
+    cases += [
+        dict(id="b-av-vec4-dense", shape=(4, 1, 4096), split=3072, dtype=F32, combine=None, next=True, out=True,
+             euler=True, tma_boundary=1, mask="rand", table="lam12"),
+        dict(id="b-av-vec4-packed-bf16", shape=(16, 1, 40960), split=30720, dtype=BF16, combine=None, next=True,
+             out=True, euler=True, packed=True, tma_boundary=1, mask="rand", table="dt"),
+        dict(id="b-av-scalar-dense-f16", shape=(3, 1, 2049), split=1000, dtype=F16, combine=None, next=True, out=True,
+             euler=True, mask="rand", table="lam01"),
+        dict(id="b-av-scalar-packed-cfg", shape=(4, 1, 4096), split=3071, dtype=F32, combine=3.5, next=True,
+             out=True, euler=True, packed=True, mask="rand", table="lam12"),
+        dict(id="b-av-big-cfg", shape=(1, 1, BIG), split=BIG // 2, dtype=F32, combine=4.5, next=True, out=True,
+             euler=True, tma_boundary=1, mask="rand", table="lam12"),
+        dict(id="b-av-split-nlast", shape=(4, 1, 4096), split=4096, dtype=F32, combine=None, next=True, out=False,
+             euler=True, tma_boundary=1, mask="rand", table="dt"),
+    ]
     for j, c in enumerate(cases):
         c.setdefault("seed", 950 + j)
     return cases
@@ -574,9 +709,10 @@ def expect_boundary(c, shape, rs, cs):
     sp, total = int(np.prod(shape[2:])), int(np.prod(shape))
     per_row = total // shape[0]
     H = DTYPES[c["dtype"]]
-    v4 = per_row % 4 == 0 and sp % 4 == 0 and rs % 4 == 0 and cs % 4 == 0 and c.get("misalign") is None
+    v4 = (per_row % 4 == 0 and sp % 4 == 0 and rs % 4 == 0 and cs % 4 == 0 and c.get("misalign") is None
+          and (c.get("split") or 0) % 4 == 0)
     tma = (v4 and c.get("tma_boundary", 0) and c["euler"] and sp % 16 == 0 and rs % 16 == 0 and cs % 16 == 0
-           and total >= TMA_MIN)
+           and total >= TMA_MIN and not c.get("split"))
     if tma:
         return f"boundary_tma_kernel<{H},{int(c['combine'] is not None)},{int(c['next'])},2048,2>"
     return f"boundary_kernel<{4 if v4 else 1},{H},{int(bool(c.get('packed')))}>"
@@ -592,8 +728,8 @@ def test_boundary_launch(c, cuda_device, options):
     total = int(np.prod(shape))
     gen = torch.Generator(device=dev).manual_seed(c["seed"])
     m8, known, rs, cs = make_mask(shape, c["mask"], gen, dev)
-    dims = dims_of(shape, rs, cs)
-    tab = make_table(shape[0], c["table"], c["seed"], dev)
+    dims = dims_of(shape, rs, cs, c.get("split"))
+    tab, rows = case_table(c, shape, dev)
     a32, b32, y, nz, x = (torch.randn(shape, device=dev, generator=gen) for _ in range(5))
     a, b = a32.to(c["dtype"]), b32.to(c["dtype"])
     nz = offset_copy(nz, 4 if c.get("misalign") == "noise" else 0)
@@ -620,8 +756,8 @@ def test_boundary_launch(c, cuda_device, options):
                                    P(m8.data_ptr()), xp, P(out.data_ptr()) if out is not None else None,
                                    C.c_float(coef), nt, C.byref(dims), _stream())
     want = R.boundary(a, b if cfg is not None else None, y, nz if c["next"] else None, known,
-                      x_in if c["euler"] else None, coef, tab if c["next"] else None, cfg=cfg)
-    got = launched(call)
+                      x_in if c["euler"] else None, coef, tab if c["next"] else None, cfg=cfg, rows=rows)
+    got = launched(call, c.get("split"))
     fam = family(want_name)
     if out is not None:
         assert torch.equal(_bits(out[known]), _bits(y[known])), f"{c['id']}: out != y at known positions"
@@ -639,28 +775,43 @@ def test_boundary_launch(c, cuda_device, options):
 # ---------------------------------------------------------------------------------------------------------------
 # lp_prologue_f32, lp_advance_f32, lp_stop_stats_f32
 # ---------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("shape,mask,copy", [((1, 4, 128, 128), "full", True), ((2, 4, 45, 45), "rand", False),
-                                            ((5, 4, 120, 136), "blob", True)])
-@rerun_on_lost_record
-def test_prologue_launch(shape, mask, copy, cuda_device):
+def _prologue(shape, mask, copy, dev, split=None):
     lib = _lib()
-    dev = cuda_device
     gen = torch.Generator(device=dev).manual_seed(77)
     m8, known, rs, cs = make_mask(shape, mask, gen, dev)
-    dims = dims_of(shape, rs, cs)
-    tab = make_table(shape[0], "lam12", 3, dev)
+    dims = dims_of(shape, rs, cs, split)
+    tab, rows = case_table(dict(table="lam12", seed=3, split=split), shape, dev)
     x, y, nz = (torch.randn(shape, device=dev, generator=gen) for _ in range(3))
     xm = torch.full(shape, float("nan"), device=dev)
     xc = torch.full(shape, float("nan"), device=dev) if copy else None
     got = launched(lambda: lib.lp_prologue_f32(P(x.data_ptr()), P(y.data_ptr()), P(nz.data_ptr()), P(m8.data_ptr()),
                                                P(xm.data_ptr()), P(xc.data_ptr()) if copy else None, P(tab.data_ptr()),
-                                               C.byref(dims), _stream()))
+                                               C.byref(dims), _stream()), split)
     assert torch.equal(_bits(xm[~known]), _bits(x[~known])), "the replace step touched free positions"
-    _check("prologue_kernel", f"prologue {shape}", xm, R.prologue(x, y, nz, known, tab))
+    _check("prologue_kernel", f"prologue {shape} split {split}", xm, R.prologue(x, y, nz, known, tab, rows=rows))
     if copy:
         assert torch.equal(_bits(xc), _bits(xm))
-    assert_kernel(f"prologue{shape}", got, f"prologue_kernel<{4 if shape[-1] % 4 == 0 else 1}>")
-    RAN.add(f"prologue{shape}")
+    v4 = shape[-1] % 4 == 0 and (split or 0) % 4 == 0
+    cid = f"prologue{shape}" + (f"-split{split}" if split is not None else "")
+    assert_kernel(cid, got, f"prologue_kernel<{4 if v4 else 1}>")
+    RAN.add(cid)
+
+
+@pytest.mark.parametrize("shape,mask,copy", [((1, 4, 128, 128), "full", True), ((2, 4, 45, 45), "rand", False),
+                                            ((5, 4, 120, 136), "blob", True)])
+@rerun_on_lost_record
+def test_prologue_launch(shape, mask, copy, cuda_device):
+    _prologue(shape, mask, copy, cuda_device)
+
+
+AV_PROLOGUE = [((4, 1, 4096), 3072, True), ((3, 1, 2049), 1000, False), ((4, 1, 4096), 3071, False)]
+
+
+@pytest.mark.parametrize("shape,split,copy", AV_PROLOGUE)
+@rerun_on_lost_record
+def test_av_prologue_launch(shape, split, copy, cuda_device):
+    """The replace step of an audio-video pack: rep_noise / rep_y of each element's own row (audio or video)."""
+    _prologue(shape, "rand", copy, cuda_device, split)
 
 
 ADVANCE = [
@@ -670,6 +821,11 @@ ADVANCE = [
     dict(id="adv-torch-pastcap", shape=(1, 4, 272, 256), rng="torch", half=1, mask="rand"),
     dict(id="adv-torch-wan", shape=(1, 16, 21, 80, 45), rng="torch", half=0, mask="full"),
     dict(id="adv-torch-flagship-state", shape=(128, 4, 128, 128), rng="torch_state", half=1, mask="rand"),
+    # audio-video flat packs
+    dict(id="adv-av-tape", shape=(4, 1, 4096), split=3072, rng="tape", half=1, mask="rand"),
+    dict(id="adv-av-philox-odd", shape=(3, 1, 2049), split=1000, rng="philox", half=0, mask="rand"),
+    dict(id="adv-av-torch-16", shape=(16, 1, 40960), split=30720, rng="torch", half=1, mask="rand"),
+    dict(id="adv-av-torch-state-big", shape=(1, 1, BIG), split=BIG // 2 + 1, rng="torch_state", half=0, mask="rand"),
 ]
 
 
@@ -684,8 +840,8 @@ def test_advance_launch(c, cuda_device, normal_fast):
     total = int(np.prod(shape))
     gen = torch.Generator(device=dev).manual_seed(len(c["id"]) * 131)
     m8, known, rs, cs = make_mask(shape, c["mask"], gen, dev)
-    dims = dims_of(shape, rs, cs)
-    tab = make_table(shape[0], "dt" if c["half"] else "lam12", 5, dev)
+    dims = dims_of(shape, rs, cs, c.get("split"))
+    tab, rows = case_table(dict(table="dt" if c["half"] else "lam12", seed=5, split=c.get("split")), shape, dev)
     x, cc = torch.randn(shape, device=dev, generator=gen) * 2, torch.randn(shape, device=dev, generator=gen) * 3
     r, keep, slack, seed = _native.Rng(), [], 0.0, 4242
     if c["rng"] == "tape":
@@ -701,7 +857,8 @@ def test_advance_launch(c, cuda_device, normal_fast):
             keep.append(st)
             r.seed, r.state = 0, st.data_ptr()
         want_name = "advance_kernel<1>"
-        sd = R._cls(tab, known, R.C_SH if c["half"] else R.C_SF, len(shape)).abs() * R._row(tab, R.T_S, len(shape)).abs()
+        nd = len(shape)
+        sd = R._cls(tab, known, R.C_SH if c["half"] else R.C_SF, nd, rows).abs() * R._row(tab, R.T_S, nd, rows).abs()
         slack = sd * normal_fast[1]
     else:
         base = 4 * 1001 if c["rng"] == "torch_state" else 0
@@ -714,12 +871,35 @@ def test_advance_launch(c, cuda_device, normal_fast):
             keep.append(st)
             r.seed, r.state, r.draw0 = 0, st.data_ptr(), 0
         want_name = "advance_torch_kernel"
-    want = R.advance(x, cc, known, tab, xi, c["half"])
+    want = R.advance(x, cc, known, tab, xi, c["half"], rows=rows)
     got = launched(lambda: lib.lp_advance_f32(P(x.data_ptr()), P(cc.data_ptr()), P(m8.data_ptr()), P(tab.data_ptr()),
-                                              C.byref(dims), C.byref(r), c["half"], _stream()))
+                                              C.byref(dims), C.byref(r), c["half"], _stream()), c.get("split"))
     _check(family(want_name), c["id"], x, want, slack=slack)
     assert_kernel(c["id"], got, want_name)
     RAN.add(c["id"])
+
+
+def _stop_stats(shape, bcast, dev, split=None):
+    lib = _lib()
+    gen = torch.Generator(device=dev).manual_seed(61)
+    m8, known, rs, cs = make_mask(shape, "rand" if bcast else "full", gen, dev)
+    ring8 = (torch.rand(m8.shape, device=dev, generator=gen) < 0.2).to(torch.uint8)
+    dims = dims_of(shape, rs, cs, split)
+    tab, rows = case_table(dict(table="lam12", seed=2, split=split), shape, dev)
+    a, b = torch.randn(shape, device=dev, generator=gen), torch.randn(shape, device=dev, generator=gen)
+    sums = torch.zeros(2, dtype=torch.float64, device=dev)
+    got = launched(lambda: lib.lp_stop_stats_f32(P(a.data_ptr()), P(b.data_ptr()), P(m8.data_ptr()),
+                                                 P(ring8.data_ptr()), P(tab.data_ptr()), C.byref(dims),
+                                                 P(sums.data_ptr()), _stream()), split)
+    want = R.stop_stats(a, b, known, ring8.bool().expand(shape), tab, rows=rows)
+    for k in range(2):
+        rel = abs(float(sums[k]) - want[k]) / want[k]
+        WORST["stop_stats_kernel"] = max(WORST["stop_stats_kernel"], rel / R.U32)
+        assert rel <= 48 * R.U32, (k, float(sums[k]), want[k])
+    v4 = shape[-1] % 4 == 0 and (split or 0) % 4 == 0
+    cid = f"stats{shape}" + (f"-split{split}" if split is not None else "")
+    assert_kernel(cid, got, f"stop_stats_kernel<{4 if v4 else 1}>")
+    RAN.add(cid)
 
 
 @pytest.mark.parametrize("shape,bcast", [((128, 4, 128, 128), False), ((2, 4, 45, 45), True)])
@@ -728,53 +908,54 @@ def test_stop_stats_launch(shape, bcast, cuda_device):
     """lp_stop_stats_f32 with the inv_S table the engine passes and a full-shape ring, against fp64 sums.  Every
     term is non-negative, so the fp32 partial sums (a grid-stride chain of at most ~40 additions per thread, then
     the warp and block trees) stay within 48 * 2^-24 of the fp64 sum."""
-    lib = _lib()
-    dev = cuda_device
-    gen = torch.Generator(device=dev).manual_seed(61)
-    m8, known, rs, cs = make_mask(shape, "rand" if bcast else "full", gen, dev)
-    ring8 = (torch.rand(m8.shape, device=dev, generator=gen) < 0.2).to(torch.uint8)
-    dims = dims_of(shape, rs, cs)
-    tab = make_table(shape[0], "lam12", 2, dev)
-    a, b = torch.randn(shape, device=dev, generator=gen), torch.randn(shape, device=dev, generator=gen)
-    sums = torch.zeros(2, dtype=torch.float64, device=dev)
-    got = launched(lambda: lib.lp_stop_stats_f32(P(a.data_ptr()), P(b.data_ptr()), P(m8.data_ptr()),
-                                                 P(ring8.data_ptr()), P(tab.data_ptr()), C.byref(dims),
-                                                 P(sums.data_ptr()), _stream()))
-    want = R.stop_stats(a, b, known, ring8.bool().expand(shape), tab)
-    for k in range(2):
-        rel = abs(float(sums[k]) - want[k]) / want[k]
-        WORST["stop_stats_kernel"] = max(WORST["stop_stats_kernel"], rel / R.U32)
-        assert rel <= 48 * R.U32, (k, float(sums[k]), want[k])
-    assert_kernel(f"stats{shape}", got, f"stop_stats_kernel<{4 if shape[-1] % 4 == 0 else 1}>")
-    RAN.add(f"stats{shape}")
+    _stop_stats(shape, bcast, cuda_device)
+
+
+AV_STATS = [((16, 1, 40960), 30720), ((3, 1, 2049), 1000)]
+
+
+@pytest.mark.parametrize("shape,split", AV_STATS)
+@rerun_on_lost_record
+def test_av_stop_stats_launch(shape, split, cuda_device):
+    """The early-stop statistics of an audio-video pack: inv_S of each element's own row, with a ring."""
+    _stop_stats(shape, True, cuda_device, split)
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # coverage
 # ---------------------------------------------------------------------------------------------------------------
-def _required():
+KINDS = ((1, 1), (1, 0), (0, 1), (0, 0))
+
+
+def _required_split():
+    """Every instantiation a launch with a row split can reach: the LDG and torch-LDG kernels (no TMA kernel)."""
     req = set()
-    kinds = ((1, 1), (1, 0), (0, 1), (0, 0))
     for N in (4, 1):
-        for f, n in kinds:
+        for f, n in KINDS:
             req.add(("substep_kernel", f"{N},0,{f},{n},0"))
             req.add(("substep_kernel", f"{N},1,{f},{n},0"))
         req.add(("substep_kernel", f"{N},1,1,1,1"))
         req.add(("substep_kernel", f"{N},1,0,1,1"))
-    for f, n, mg in ((1, 1, 1), (1, 1, 0), (0, 1, 1), (0, 1, 0), (1, 0, 0), (0, 0, 0)):
-        req.add(("substep_tma_kernel", f"{f},{n},{mg},2048,2,2"))
-    for f, n in kinds:
-        for pk in (0, 1):
-            req.add(("substep_torch_tma_kernel", f"{f},{n},{pk}"))
+    for f, n in KINDS:
         req.add(("substep_torchvec_kernel", f"{f},{n}"))
         req.add(("substep_torch_kernel", f"{f},{n}"))
     for N in (4, 1):
         for pk in (0, 1):
             req.add(("boundary_kernel", f"{N},{pk}"))
-    req.add(("boundary_tma_kernel", None))
     for s in ("prologue_kernel<4>", "prologue_kernel<1>", "advance_kernel<0>", "advance_kernel<1>",
               "advance_torch_kernel", "stop_stats_kernel<4>", "stop_stats_kernel<1>"):
         req.add((s, ""))
+    return req
+
+
+def _required():
+    req = _required_split()
+    for f, n, mg in ((1, 1, 1), (1, 1, 0), (0, 1, 1), (0, 1, 0), (1, 0, 0), (0, 0, 0)):
+        req.add(("substep_tma_kernel", f"{f},{n},{mg},2048,2,2"))
+    for f, n in KINDS:
+        for pk in (0, 1):
+            req.add(("substep_torch_tma_kernel", f"{f},{n},{pk}"))
+    req.add(("boundary_tma_kernel", None))
     return req
 
 
@@ -792,20 +973,26 @@ def _split(name):
     return fam, args[h], ",".join(args[:h] + args[h + 1:])
 
 
-def test_kernel_coverage():
-    """The union of the kernels the cases above ran covers every production-reachable instantiation of the update
-    kernels (the measurement-only philox tile geometries, "tma" 2..5, excluded) and every head type per family."""
-    n_cases = len(SUBSTEP_CASES) + len(_boundary_sweep()) + 3 + len(ADVANCE) + 2
-    if len(RAN) < n_cases:
-        pytest.skip(f"only {len(RAN)} of the {n_cases} launch cases ran in this session")
+def _seen(counter):
     seen = set()
     heads = collections.defaultdict(set)
-    for name in SEEN:
+    for name in counter:
         fam, h, rest = _split(name)
         seen.add((fam, rest))
         seen.add((fam, None))
         if h is not None:
             heads[fam].add(h)
+    return seen, heads
+
+
+def test_kernel_coverage():
+    """The union of the kernels the cases above ran covers every production-reachable instantiation of the update
+    kernels (the measurement-only philox tile geometries, "tma" 2..5, excluded) and every head type per family; the
+    cases with a row split ran every instantiation a split can reach, and never a TMA kernel."""
+    n_cases = len(SUBSTEP_CASES) + len(_boundary_sweep()) + 3 + len(AV_PROLOGUE) + len(ADVANCE) + 2 + len(AV_STATS)
+    if len(RAN) < n_cases:
+        pytest.skip(f"only {len(RAN)} of the {n_cases} launch cases ran in this session")
+    seen, heads = _seen(SEEN)
     print("\nkernels seen (launches):")
     for name in sorted(SEEN):
         print(f"  {SEEN[name]:3d}  {name}")
@@ -814,5 +1001,10 @@ def test_kernel_coverage():
         print(f"  {fam:28s} {WORST[fam]:.3g}")
     missing = sorted(str(r) for r in _required() if r not in seen)
     assert not missing, missing
+    seen_split, _ = _seen(SEEN_SPLIT)
+    missing = sorted(str(r) for r in _required_split() if r not in seen_split)
+    print(f"row-split launches: {sum(SEEN_SPLIT.values())}, instantiations missing: {missing}")
+    assert not missing, missing
+    assert not [n for n in SEEN_SPLIT if "tma" in n], sorted(SEEN_SPLIT)
     for fam in HEAD_FAMILIES:
         assert heads[fam] == set(DTYPES.values()), (fam, heads[fam])
