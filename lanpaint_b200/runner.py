@@ -342,8 +342,8 @@ class GraphedJob:
                              None, self.rng_state.data_ptr(), euler_coef=coef if self.fused_euler else None,
                              skip_prologue=(self.fused_euler and i > 0) or (i == 0 and self.first_replace_noop),
                              next_table=self.tables[i + 1] if (self.fused_euler and not last) else None)
-        if not self.fused_euler:
-            self.x.add_(self.x - self.out, alpha=coef)
+        if not self.fused_euler:     # from this step's denoised latent, wherever it was written
+            self.x.add_(self.x - out, alpha=coef)
 
     def _body(self, plan, want_out):
         if not self.external_init:
@@ -364,11 +364,16 @@ class GraphedJob:
         plan = self._relative_plan()   # built BEFORE capture begins: reading the generator's offset is not capturable
         try:
             if warm:
+                # the warm-up pass really runs the captured steps: put the sampler state back afterwards, or an outer
+                # step captured on its own (mode "steps"), or a job whose initial state was loaded from x_init, would
+                # then be applied twice
+                state = self.x.clone()
                 side = torch.cuda.Stream(device=self.device)
                 side.wait_stream(torch.cuda.current_stream(self.device))
                 with torch.cuda.stream(side):
                     fn(plan)
                 torch.cuda.current_stream(self.device).wait_stream(side)
+                self.x.copy_(state)
                 eng.launches, eng.model_calls, eng.substeps_done = counts
             graph = torch.cuda.CUDAGraph()
             lib = _native.load()

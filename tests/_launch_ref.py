@@ -24,10 +24,22 @@ for the philox stream.
 """
 from __future__ import annotations
 
+import re
+
 import numpy as np
 import torch
 
 U32 = 2.0 ** -24   # unit round-off of fp32
+
+
+def canon(name: str) -> str:
+    """A profiler's kernel name -> the canonical spelling the tests assert on:
+    'void lp::substep_kernel<(int)4, float, (bool)1, ...>(lp::SubstepArgs)' (or the true/false spelling)
+    -> 'substep_kernel<4,float,1,...>'."""
+    n = name.split("lp::", 1)[1]
+    n = n[: n.index(">") + 1] if "<" in n.split("(")[0] else n.split("(")[0]
+    n = n.replace("(bool)", "").replace("(int)", "").replace("true", "1").replace("false", "0").replace(" ", "")
+    return re.sub(r"(\d+)u\b", r"\1", n)
 
 # table layout (include/lanpaint_b200.h)
 T_CTGT, T_S, T_INVS, T_LAM, T_ONEPLAM, T_REPN, T_REPY, T_CORR = 0, 1, 2, 3, 4, 5, 6, 7

@@ -14,6 +14,26 @@ def denoiser(x, sigma, cond):
     return 0.7 * x + 0.1 * torch.tanh(x) + cond
 
 
+def mixing_denoiser(x, sigma, cond):
+    """`denoiser` plus a fixed coupling of every element to its neighbours over channels and every spatial /
+    sequence axis (never the batch axis: requests stay independent).  With a pointwise network a free element's
+    trajectory never reads a known one, so nothing a job does at known positions reaches the final latent except the
+    paste `out = y`; with this one the known region feeds the free region through every model call.  Elementwise
+    ops and `roll` only: no TF32, the same on CPU and GPU up to a tanh ulp, capturable in a CUDA graph."""
+    out = 0.6 * x + 0.1 * torch.tanh(x) + cond
+    for d in range(1, x.ndim):
+        out = out + 0.05 * torch.roll(x, 1, d)
+    return out
+
+
+NETS = {"pointwise": denoiser, "mixing": mixing_denoiser}
+
+
+def net_of(c):
+    """The test network a case (a fixture's meta) was generated with."""
+    return NETS[c.get("net", "pointwise")]
+
+
 class FixedNoise:
     """a NOISE object for LanPaint_SamplerCustomAdvanced (ComfyUI's RandomNoise protocol: .seed, .generate_noise)"""
 
@@ -27,7 +47,10 @@ class FixedNoise:
 POS, NEG = 0.3, -0.2
 
 
-def build_patcher(c, device="cpu", net=denoiser):
+def build_patcher(c, device="cpu", net=None):
+    """`net` (a counting wrapper, say) defaults to the case's own network, `net_of(c)`."""
+    if net is None:
+        net = net_of(c)
     mtype = getattr(minicomfy.ModelType, c.get("model_type", "EPS"))
     cls = minicomfy.WAN22 if c.get("wan22") else minicomfy.BaseModel
     base = cls(net, model_type=mtype, latent_channels=c["shape"][1], shift=c.get("shift", 1.0))

@@ -1,6 +1,7 @@
 """Node-level golden vectors from the REAL reference node layer (run in the build container only).
 
-    python tests/golden/make_node_golden.py        # writes tests/golden/node_*.npz
+    python tests/golden/make_node_golden.py                  # writes tests/golden/node_*.npz
+    python tests/golden/make_node_golden.py --only '_mix$'   # writes only the fixtures whose name matches
 
 The unmodified `/root/reference/src/LanPaint/nodes.py` is imported with `minicomfy` standing in for ComfyUI and
 its four sampler nodes are driven on the CPU, from the LATENT dict in to the LATENT dict out: common_ksampler /
@@ -19,6 +20,7 @@ from __future__ import annotations
 import importlib
 import json
 import os
+import re
 import sys
 import warnings
 from unittest import mock
@@ -35,7 +37,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import minicomfy  # noqa: E402
 from _node_cases import (FixedNoise, IMAGE_MODE, NEG, POS, VIDEO_MODE, build_patcher, call_node,  # noqa: E402
-                         denoiser)
+                         net_of)
 
 
 class Fp16Tape:
@@ -102,6 +104,14 @@ CASES = [
 ]
 
 
+# the same calls with a network that couples positions (`_node_cases.mixing_denoiser`): only with it do the settings
+# that act at known positions (cfg_BIG / prompt mode, lambda, the noise image, add_noise) reach the output latent
+MIXED = ("node_ksampler_sdxl_karras20_n5", "node_ksampler_prompt_first_batch2", "node_ksampler_flux_simple",
+         "node_ksampler_flow_video", "node_ksampler_heun", "node_advanced_window_leftover", "node_advanced_noise_disabled",
+         "node_custom_random_noise", "node_av_flat_pack")
+CASES += [dict(c, name=c["name"] + "_mix", net="mixing") for c in CASES if c["name"] in MIXED]
+
+
 def case_inputs(c):
     g = torch.Generator().manual_seed(100 + len(c["name"]))
     y = torch.randn(c["shape"], generator=g)
@@ -111,7 +121,12 @@ def case_inputs(c):
     return latent
 
 
-def main():
+def main(argv=None):
+    import argparse
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--only", metavar="REGEX", help="write only the fixtures whose name matches (re.search); the "
+                    "others stay untouched (rewriting one changes its zip timestamps even when the arrays do not)")
+    args = ap.parse_args(argv)
     warnings.filterwarnings("ignore")
     torch.set_num_threads(1)
     minicomfy.install()
@@ -119,12 +134,14 @@ def main():
     assert ref.__file__.startswith("/root/reference/"), ref.__file__
     real_prepare_noise = minicomfy.prepare_noise
     for c in CASES:
+        if args.only is not None and not re.search(args.only, c["name"]):
+            continue
         latent = case_inputs(c)
         calls = {"n": 0}
 
         def net(x, sigma, cond):
             calls["n"] += 1
-            return denoiser(x, sigma, cond)
+            return net_of(c)(x, sigma, cond)
 
         patcher = build_patcher(c, net=net)
         tape = Fp16Tape(seed=4321 + len(c["name"]))

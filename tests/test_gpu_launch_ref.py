@@ -40,7 +40,6 @@ MinStepFrac 0, Lambda 0.1 or 12 and Beta 1.5 (distinct dt per mask class), or co
 import collections
 import ctypes as C
 import functools
-import re
 import time
 
 import numpy as np
@@ -76,13 +75,7 @@ def _stream():
 # ---------------------------------------------------------------------------------------------------------------
 # which kernel ran
 # ---------------------------------------------------------------------------------------------------------------
-def canon(name: str) -> str:
-    """'void lp::substep_kernel<(int)4, float, (bool)1, ...>(lp::SubstepArgs)' (or the true/false spelling)
-    -> 'substep_kernel<4,float,1,...>'."""
-    n = name.split("lp::", 1)[1]
-    n = n[: n.index(">") + 1] if "<" in n.split("(")[0] else n.split("(")[0]
-    n = n.replace("(bool)", "").replace("(int)", "").replace("true", "1").replace("false", "0").replace(" ", "")
-    return re.sub(r"(\d+)u\b", r"\1", n)
+canon = R.canon
 
 
 class LostRecord(Exception):

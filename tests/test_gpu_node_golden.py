@@ -8,7 +8,9 @@ compared is everything between the two LATENT dicts: mask preparation, noise sca
 glue, the inner-step ramp, dual CFG, the fused update kernels, the sampler's own steps and the epilogue
 (nodes.py:161-216, 229-379, 487-513).  Tolerance: the north_star contract (1e-3 of the final latent's scale)
 with fp32 round-off asserted at 5e-6 (the network stand-in's tanh differs by an ulp between CPU and GPU).  `node_av_flat_pack` enters at the patched CFGGuider.outer_sample with `latent_shapes`, the way ComfyUI
-hands over a nested (video, audio) latent (MiniMax-H3: audio rows on their own shifted sigma schedule)."""
+hands over a nested (video, audio) latent (MiniMax-H3: audio rows on their own shifted sigma schedule).
+The `*_mix` fixtures run the same calls with `_node_cases.mixing_denoiser`, a network that couples positions, so that
+what the node layer does at known positions (cfg_BIG, lambda, the replace step, the noise image) reaches `out`."""
 import glob
 import json
 import os
@@ -20,7 +22,7 @@ import pytest
 import torch
 
 import minicomfy
-from _node_cases import build_patcher, call_node, denoiser
+from _node_cases import build_patcher, call_node, net_of
 from _support import max_rel
 from conftest import GOLDEN_DIR
 
@@ -58,7 +60,7 @@ def test_node_matches_reference_node_layer(name, cuda_device):
 
     def net(x, sigma, cond):
         calls["n"] += 1
-        return denoiser(x, sigma, cond)
+        return net_of(c)(x, sigma, cond)
 
     patcher = build_patcher(c, device=dev, net=net)
     tape = NoiseTape([torch.from_numpy(t.astype(np.float32)) for t in g["tape"]])
@@ -119,7 +121,7 @@ def test_engine_seam_under_the_reference_node_layer(name, cuda_device, monkeypat
 
     def net(x, sigma, cond):
         calls["n"] += 1
-        return denoiser(x, sigma, cond)
+        return net_of(c)(x, sigma, cond)
 
     patcher = build_patcher(c, device=dev, net=net)
     tape = NoiseTape([torch.from_numpy(t.astype(np.float32)) for t in g["tape"]])

@@ -50,7 +50,8 @@ def test_reference_bytecode_node_layer_reproduces_the_node_goldens(monkeypatch):
     if ref_nodes is None:
         pytest.skip("oracle/_ref not built (needs /root/reference: `make -C oracle`)")
     assert ref_nodes.__file__.endswith(".pyc")
-    for name in ("node_ksampler_prompt_first_batch2", "node_advanced_window_leftover", "node_custom_random_noise"):
+    for name in ("node_ksampler_prompt_first_batch2", "node_advanced_window_leftover", "node_custom_random_noise",
+                 "node_advanced_window_leftover_mix"):
         z = np.load(os.path.join(GOLDEN_DIR, name + ".npz"))
         c = json.loads(str(z["meta"]))
         replay = iter(torch.from_numpy(t.astype(np.float32)) for t in z["tape"])
