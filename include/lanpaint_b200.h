@@ -137,7 +137,7 @@ int lp_abi_version(void);
 const char* lp_status_string(int status);
 int lp_last_cuda_error(void); /* cudaError_t of the last failed launch on this thread */
 /* Process-wide switches (also read once from the environment: LANPAINT_B200_PDL, LANPAINT_B200_TMA,
- * LANPAINT_B200_TMA_MIN, LANPAINT_B200_TMA_BOUNDARY):
+ * LANPAINT_B200_TMA_MIN, LANPAINT_B200_TMA_BOUNDARY, LANPAINT_B200_L2_HANDOFF):
  *   "pdl" 1|0      programmatic dependent launch on every kernel (default 1)
  *   "tma" 1|0      use the TMA-staged persistent variants (cp.async.bulk + mbarrier ring) of the fused sub-step
  *                  (philox and torch streams) and of the step-boundary kernel when eligible: spatial a multiple
@@ -145,7 +145,11 @@ int lp_last_cuda_error(void); /* cudaError_t of the last failed launch on this t
  *                  the philox kernel, for measurement)
  *   "tma_min"      smallest launch, in elements, that takes a TMA-staged variant (default 2^18)
  *   "tma_boundary" 1|0  lp_boundary: TMA-staged kernel when eligible | always the LDG kernel (default 0: measured
- *                  faster inside a job, where the network's output is still in L2) */
+ *                  faster inside a job, where the network's output is still in L2)
+ *   "l2_handoff"   bits, for measurement: 1 the TMA sub-steps and the step-boundary kernels walk their launch
+ *                  tail-first, 2 evict-first L2 policy on the heads, C and the boundary's output (default 3);
+ *                  launches of fewer than 2^20 elements, whose job stays in L2, use neither.  Results do not
+ *                  depend on it. */
 int lp_set_option(const char* name, int value);
 
 /* Host-only self test of the index arithmetic the kernels rely on (the multiply-shift division that

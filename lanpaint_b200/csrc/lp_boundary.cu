@@ -49,6 +49,7 @@ struct BoundaryArgs {
   const float* next_table;  // NULL: no replace step of the next outer step
   float cfg, coef;
   int combine;
+  int l2;          // kL2* bits of this launch (l2_handoff)
   Geometry g;
 };
 
@@ -68,8 +69,9 @@ __device__ __forceinline__ void boundary_element(float a, float b, float y, floa
 template <int N, typename H, bool kPk>
 __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) {
   pdl_prologue();
-  const uint32_t i = (blockIdx.x * kBlock + threadIdx.x) * N;
+  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
   if (i >= p.g.total) return;
+  const uint64_t dead = l2_policy_dead(p.l2);
   uint32_t row, mi;
   locate(p.g, i, row, mi);
   const bool euler = p.x != nullptr, next = p.next_table != nullptr;
@@ -108,8 +110,8 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
   }
   // free positions: the denoised output and the running state; known positions: the re-noised clean latent
   if (any_free) {
-    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av);
-    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv);
+    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
+    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
   }
   if (euler && (any_free || !next)) load_f<N>(p.x, i, xv);
   float rn = 0.f, ry = 0.f;
@@ -130,7 +132,7 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
   for (int j = 0; j < N; ++j)
     boundary_element(av[j], bv[j], yv[j], nv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, p.coef, euler, next, rn,
                      ry);
-  if (p.out) store_f<N>(p.out, i, ov);
+  if (p.out) store_f<N>(p.out, i, ov, dead);
   if (euler) store_f<N>(p.x, i, xv);
 }
 
@@ -157,6 +159,7 @@ __global__ void __launch_bounds__(kBlock, 2) boundary_tma_kernel(const BoundaryA
   const uint32_t S = p.g.spatial.d;
   const H* ap = static_cast<const H*>(p.a);
   const H* bp = static_cast<const H*>(p.b);
+  const uint64_t dead = l2_policy_dead(p.l2);
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int s = 0; s < kStages; ++s) mbar_init(&full[s], 1);
@@ -164,6 +167,7 @@ __global__ void __launch_bounds__(kBlock, 2) boundary_tma_kernel(const BoundaryA
   }
   __syncthreads();
   auto tile_origin = [&](uint32_t tile, uint32_t& e0, uint32_t& len, uint32_t& row, uint32_t& mi0) {
+    tile = walk_index(p.l2, tile, tg.n_tiles);  // `tile` counts in walk order
     const uint32_t rc = tile / tg.tiles_per_channel;
     const uint32_t s0 = (tile - rc * tg.tiles_per_channel) * kTile;
     len = S - s0 < (uint32_t)kTile ? S - s0 : (uint32_t)kTile;
@@ -177,8 +181,8 @@ __global__ void __launch_bounds__(kBlock, 2) boundary_tma_kernel(const BoundaryA
     const uint32_t fb = len * 4u, hb = len * (uint32_t)sizeof(H);
     mbar_expect_tx(&full[s], fb * (2u + (kNext ? 1u : 0u)) + hb * (1u + (kCombine ? 1u : 0u)) + len);
     Stage& t = stage[s];
-    tma_load_1d(t.a, ap + e0, hb, &full[s]);
-    if (kCombine) tma_load_1d(t.b, bp + e0, hb, &full[s]);
+    tma_load_1d(t.a, ap + e0, hb, &full[s], dead);
+    if (kCombine) tma_load_1d(t.b, bp + e0, hb, &full[s], dead);
     tma_load_1d(t.y, p.y + e0, fb, &full[s]);
     if (kNext) tma_load_1d(t.nz, p.noise + e0, fb, &full[s]);
     tma_load_1d(t.x, p.x + e0, fb, &full[s]);
@@ -221,7 +225,7 @@ __global__ void __launch_bounds__(kBlock, 2) boundary_tma_kernel(const BoundaryA
         for (int j = 0; j < 4; ++j)
           boundary_element(av[j], bv[j], y[j], nz[j], known[j], x[j], o[j], kCombine, p.cfg, p.coef, true, kNext, rn, ry);
         const uint32_t i = e0 + 4 * v;
-        if (p.out) *reinterpret_cast<float4*>(p.out + i) = make_float4(o[0], o[1], o[2], o[3]);
+        if (p.out) st_f4(p.out + i, make_float4(o[0], o[1], o[2], o[3]), dead);
         *reinterpret_cast<float4*>(p.x + i) = make_float4(x[0], x[1], x[2], x[3]);
       }
     }
@@ -285,6 +289,7 @@ static int boundary_impl(const lp_heads* mo, const float* y, const float* noise,
   p.a = mo->a; p.b = mo->combine ? mo->b : nullptr; p.y = y; p.noise = noise; p.mask = mask; p.x = x_inout; p.out = out;
   p.kwords = known ? known->words : nullptr; p.yk = known ? known->y : nullptr; p.nk = known ? known->noise : nullptr;
   p.next_table = next_table; p.cfg = mo->cfg; p.coef = euler_coef; p.combine = mo->combine != 0;
+  p.l2 = l2_handoff(p.g.total);
   const bool v4 = geometry_vec4(p.g, mask) && head_aligned(p.a, dtype) && (!p.b || head_aligned(p.b, dtype)) &&
                   aligned16(y) && (!noise || aligned16(noise)) && (!x_inout || aligned16(x_inout)) &&
                   (!out || aligned16(out));

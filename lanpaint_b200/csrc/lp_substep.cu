@@ -34,6 +34,7 @@ struct SubstepArgs {
   uint32_t torch_T;  // threads of torch's randn grid (LP_RNG_TORCH)
   int store_c;       // write C even when the next half-advance is not fused
   int use_cfg;       // x0/x0b hold raw cond/uncond predictions: combine them here
+  int l2;            // kL2* bits of this launch (l2_handoff)
   float cfg, cfg_big;
 };
 
@@ -158,6 +159,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) substep_tma_kernel(const S
   const bool aliased = a.x0b == a.x0;
   const H* x0p = static_cast<const H*>(a.x0);
   const H* x0bp = static_cast<const H*>(a.x0b);
+  const uint64_t dead = l2_policy_dead(a.l2);
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int s = 0; s < kStages; ++s) mbar_init(&full[s], 1);
@@ -165,7 +167,9 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) substep_tma_kernel(const S
   }
   __syncthreads();
 
+  // `tile` counts in walk order; issue and consume map it to the same tile
   auto tile_origin = [&](uint32_t tile, uint32_t& e0, uint32_t& len, uint32_t& row, uint32_t& mi0) {
+    tile = walk_index(a.l2, tile, tg.n_tiles);
     const uint32_t rc = tile / tg.tiles_per_channel;          // row * channels + channel
     const uint32_t s0 = (tile - rc * tg.tiles_per_channel) * kTile;
     len = S - s0 < (uint32_t)kTile ? S - s0 : (uint32_t)kTile;
@@ -181,10 +185,10 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) substep_tma_kernel(const S
     mbar_expect_tx(&full[s], total);
     Stage& t = stage[s];
     tma_load_1d(t.x, a.x + e0, fb, &full[s]);
-    tma_load_1d(t.x0, x0p + e0, hb, &full[s]);
-    if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[s]);
+    tma_load_1d(t.x0, x0p + e0, hb, &full[s], dead);
+    if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[s], dead);
     tma_load_1d(t.y, a.y + e0, fb, &full[s]);
-    if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[s]);
+    if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[s], dead);
     tma_load_1d(t.m, a.mask + mi0, len, &full[s]);
   };
 
@@ -243,7 +247,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) substep_tma_kernel(const S
           substep_element<kFirst, kNext, kMerge>(x[j], x0[j], x0b[j], y[j], cp[j], known[j], xi1[j], xi2[j], rc, cn[j],
                                                 te[j]);
         *reinterpret_cast<float4*>(a.x + i) = make_float4(x[0], x[1], x[2], x[3]);
-        if (kNext || a.store_c) *reinterpret_cast<float4*>(a.c + i) = make_float4(cn[0], cn[1], cn[2], cn[3]);
+        if (kNext || a.store_c) st_f4(a.c + i, make_float4(cn[0], cn[1], cn[2], cn[3]), dead);
       }
     }
     __syncthreads();  // every thread is done reading stage s
@@ -320,8 +324,10 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
     if (lane == 0) {
       const H* x0p = static_cast<const H*>(a.x0);
       const H* x0bp = static_cast<const H*>(a.x0b);
+      const uint64_t dead = l2_policy_dead(a.l2);
       uint32_t it = 0;
-      for (uint32_t grp = blockIdx.x; grp < tg.n_groups; grp += gridDim.x, ++it) {
+      for (uint32_t step = blockIdx.x; step < tg.n_groups; step += gridDim.x, ++it) {
+        const uint32_t grp = walk_index(a.l2, step, tg.n_groups);  // the consumers map `step` the same way
         const uint32_t k = grp / tg.groups_per_call, b = grp - k * tg.groups_per_call;
         uint32_t lo[4] = {0u, 0u, 0u, 0u}, hi[4] = {0u, 0u, 0u, 0u};
         if constexpr (kPk) {  // the packed-y spans of the group: loaded before the first slot wait, which hides them
@@ -352,19 +358,19 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
             mbar_expect_tx(&full[j], len ? fb * (1u + (kFirst ? 0u : 1u)) + heads + yb + nw * 8u : 0u);
             if (len == 0) continue;
             tma_load_1d(t.x, a.x + e0, fb, &full[j]);
-            tma_load_1d(t.x0, x0p + e0, hb, &full[j]);
-            if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j]);
+            tma_load_1d(t.x0, x0p + e0, hb, &full[j], dead);
+            if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j], dead);
             if (yb) tma_load_1d(t.y, a.yk + ylo, yb, &full[j]);
-            if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j]);
+            if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j], dead);
             tma_load_1d(t.w, a.kwords + 2u * (e0 >> 5), nw * 8u, &full[j]);
           } else {
             mbar_expect_tx(&full[j], fb * (2u + (kFirst ? 0u : 1u)) + heads + len);
             if (len == 0) continue;
             tma_load_1d(t.x, a.x + e0, fb, &full[j]);
-            tma_load_1d(t.x0, x0p + e0, hb, &full[j]);
-            if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j]);
+            tma_load_1d(t.x0, x0p + e0, hb, &full[j], dead);
+            if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j], dead);
             tma_load_1d(t.y, a.y + e0, fb, &full[j]);
-            if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j]);
+            if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j], dead);
             // the mask is indexed per (row, channel): one slice per channel segment the sub-tile touches
             uint32_t e = e0, off = 0, rem = len;
             while (rem) {
@@ -418,7 +424,8 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
       cn[q] = cc[0]; cn[q + 1] = cc[1];
     }
     *reinterpret_cast<float4*>(a.x + i) = make_float4(x[0], x[1], x[2], x[3]);
-    if (kNext || a.store_c) *reinterpret_cast<float4*>(a.c + i) = make_float4(cn[0], cn[1], cn[2], cn[3]);
+    // the policy is made where it is used: held across the loop it costs the consumers a spill
+    if (kNext || a.store_c) st_f4(a.c + i, make_float4(cn[0], cn[1], cn[2], cn[3]), l2_policy_dead(a.l2));
   };
   auto fetch = [&](const Slot& t, float (&x)[4], float (&x0)[4], float (&x0b)[4], float (&y)[4], float (&cp)[4],
                    uint32_t& kb) {
@@ -449,7 +456,8 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
   // the producer's next cp.async.bulk; with per-thread arrives it reports none.)
   auto release = [&](int j) { mbar_arrive(&empty[j]); };
   uint32_t it = 0;
-  for (uint32_t grp = blockIdx.x; grp < tg.n_groups; grp += gridDim.x, ++it) {
+  for (uint32_t step = blockIdx.x; step < tg.n_groups; step += gridDim.x, ++it) {
+    const uint32_t grp = walk_index(a.l2, step, tg.n_groups);
     const uint32_t k = grp / tg.groups_per_call, b = grp - k * tg.groups_per_call;
     const uint32_t t0 = b * kG + 4u * tid;  // my four Philox subsequences (torch threads)
     // all four planes complete (every group but those at the very end of the tensor): no per-thread predicates
@@ -762,6 +770,7 @@ static int substep_impl(float* x_model, const lp_heads* heads, const float* y, c
   a.seed = rng->seed; a.draw0 = rng->draw0; a.draw1 = rng->draw1; a.torch_T = 0;
   a.store_c = (flags & LP_SUBSTEP_STORE_C) != 0;
   a.use_cfg = heads->combine != 0; a.cfg = heads->cfg; a.cfg_big = heads->cfg_big;
+  a.l2 = l2_handoff(a.g.total);
   cudaStream_t s = (cudaStream_t)stream;
   const bool v4 = geometry_vec4(a.g, mask) && aligned16(x_model) && head_aligned(x0, dtype) &&
                   head_aligned(x0_big, dtype) && aligned16(y) && (!c_state || aligned16(c_state)) &&
