@@ -14,7 +14,9 @@ production runs, and each case asserts which sub-step kernel that was.
 
 Each case asserts: max|got - want| <= B * max|want| on the final latent and on every step's denoised latent (where
 a callback exists), whose known positions must equal y bit for bit; and the generator offset after the job equals the
-reference's."""
+reference's.  Besides the plain Euler KSampler the node routes users reach are covered: a KSamplerAdvanced window
+with leftover noise, add_noise = disable, denoise < 1, euler_ancestral, SamplerCustomAdvanced on Flux (both outputs),
+an audio-video pack through `outer_sample(latent_shapes=...)` and the inner early stop."""
 import collections
 import json
 import sys
@@ -26,7 +28,7 @@ from torch.profiler import ProfilerActivity, profile
 import _job_ref as J
 import minicomfy
 from _launch_ref import canon
-from _node_cases import NEG, POS, mixing_denoiser
+from _node_cases import NEG, POS, FixedNoise, av_shift_sigma, av_shift_slope, mixing_denoiser
 from oracle import langevin_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -59,13 +61,18 @@ def _check_steps(case, label, got_steps, want_steps, y, known):
         assert torch.equal(d[known], y[known]), f"{case} {label}: denoised[{i}] differs from y at a known position"
 
 
-def _sub_kernels(fn):
-    """Run fn() under torch.profiler -> (its result, the canonical names of the sub-step kernels it launched)."""
+def _lp_kernels(fn):
+    """Run fn() under torch.profiler -> (its result, the canonical names of the library kernels it launched)."""
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         out = fn()
         torch.cuda.synchronize()
-    names = {canon(e.name()) for e in prof.profiler.kineto_results.events() if "lp::" in e.name()}
+    return out, {canon(e.name()) for e in prof.profiler.kineto_results.events() if "lp::" in e.name()}
+
+
+def _sub_kernels(fn):
+    """Run fn() under torch.profiler -> (its result, the canonical names of the sub-step kernels it launched)."""
+    out, names = _lp_kernels(fn)
     return out, {n for n in names if n.startswith("substep")}
 
 
@@ -74,6 +81,13 @@ def _assert_torch_tma(case, names, packed):
     assert names, f"{case}: no sub-step kernel recorded"
     bad = [n for n in names if not (n.startswith("substep_torch_tma_kernel<") and n.endswith(f",{int(packed)}>"))]
     assert not bad, (case, sorted(names))
+
+
+def _assert_family(case, names, family):
+    """Every sub-step launch ran one kernel family (a side output or a row split rules the TMA kernels out)."""
+    subs = {n for n in names if n.startswith("substep")}
+    assert subs, f"{case}: no sub-step kernel recorded"
+    assert all(n.startswith(family + "<") for n in subs), (case, sorted(subs))
 
 
 def _blob(shape, gen):
@@ -112,6 +126,8 @@ def _recorder(store):
     def prepare_callback(model, steps, x0_output_dict=None):
         def callback(step, x0, x, total_steps):
             store.append((step, x0.detach().clone()))
+            if x0_output_dict is not None:      # the custom-sampler nodes' denoised_output
+                x0_output_dict["x0"] = x0
         return callback
     return prepare_callback
 
@@ -121,10 +137,12 @@ def _recorder(store):
 # ---------------------------------------------------------------------------------------------------------------
 NODE = dict(shape=(8, 4, 128, 128), mask="rand", mode="Image First", steps=20, n=5, cfg=5.0, sampler="euler",
             scheduler="karras", model_type="EPS", shift=1.0, wan22=False, opts=None, calls=2,
-            modes=None, packed=(True, True))
+            modes=None, packed=(True, True), denoise=1.0, window=None, add_noise=True, lam=5.0, step_size=0.2)
 # packed: the operands the (first, last) call's sub-steps read.  The fused Euler loop (GraphedJob) and the
 # whole-sampler graph (SamplerGraphJob) build the packed known-operand layout once per job; the per-sigma path
 # (the engine behind k-diffusion's own loop, and the eager job a SamplerGraphJob records) reads the dense operands.
+# window: (start_at_step, end_at_step, return_with_leftover_noise) -- the case calls LanPaint_KSamplerAdvanced, with
+# add_noise, lam and step_size as its widgets; otherwise LanPaint_KSampler with `denoise`.
 NODE_CASES = {}
 for _m in ("rand", "rand1"):
     for _p in ("Image First", "Prompt First"):
@@ -148,6 +166,18 @@ NODE_CASES.update({
                              modes=["steps", "steps", "job"]),
     "b8-heun-sampler-graph": dict(NODE, sampler="heun", steps=10, calls=3, opts={"deferred_max_ms": 1e9},
                                   modes=[None, "sampler-graph", "sampler-graph"], packed=(False, True)),
+    # a step window that returns its leftover noise: the fused loop's last boundary steps to sigma > 0, no
+    # max_denoise, the inner-step ramp over a truncated schedule, lambda and step size from the widgets
+    "adv-window-leftover": dict(NODE, window=(3, 15, True), lam=8.0, step_size=0.15, calls=4),
+    "adv-window-leftover-r128": dict(NODE, shape=(128, 4, 128, 128), window=(3, 15, True), lam=8.0, step_size=0.15,
+                                     calls=3),
+    # add_noise = disable: a fresh noise image from the generator at every outer step, before that step's Langevin
+    # draws -- k-diffusion's loop around the per-sigma graphs, dense operands
+    "adv-noise-disabled": dict(NODE, window=(2, 10000, False), add_noise=False, mode="Prompt First", calls=4,
+                               modes=[None] * 4, packed=(False, False)),
+    "denoise-0.6": dict(NODE, denoise=0.6, calls=4),
+    # the sampler draws its own noise between wrapper calls: per-sigma graphs, never a whole-loop graph
+    "euler-ancestral": dict(NODE, sampler="euler_ancestral", calls=4, modes=[None] * 4, packed=(False, False)),
 })
 
 
@@ -171,10 +201,14 @@ def test_ksampler_job_matches_fp64(case, cuda_device, monkeypatch):
     monkeypatch.setattr(sys.modules["latent_preview"], "prepare_callback", _recorder(store))
     flow = c["model_type"] in ("FLUX", "FLOW")
     sampling = O.FlowSampling() if flow else O.VESampling()
-    sig = minicomfy.KSampler(patcher, c["steps"], dev, c["sampler"], c["scheduler"]).sigmas
+    window = {}
+    if c["window"] is not None:
+        start, end, leftover = c["window"]
+        window = dict(start_step=start, last_step=end, force_full_denoise=not leftover)
+    sig = J.ksampler_sigmas(patcher, c["steps"], c["sampler"], c["scheduler"], c["denoise"], **window)
     md = J.max_denoise(base.model_sampling, sig[0])
     cfg_big = 1.0 if c["model_type"] == "FLUX" else (c["cfg"] if c["mode"] == "Image First" else -0.5)
-    hp = O.Hyper(n_steps=c["n"], min_step_frac=1.0, flow=flow)
+    hp = O.Hyper(n_steps=c["n"], lam=c["lam"], step_size=c["step_size"], min_step_frac=1.0, flow=flow)
     g = torch.Generator().manual_seed(sum(map(ord, case)))
     y = torch.randn(shape, generator=g)
     mask = _mask(c["mask"], shape, g)
@@ -185,11 +219,19 @@ def test_ksampler_job_matches_fp64(case, cuda_device, monkeypatch):
         if k == 3:
             y, mask = torch.randn(shape, generator=g), _mask(c["mask"], shape, g)
         store.clear()
+        latent = {"samples": y, "noise_mask": mask}
 
         def call():
-            (out,) = N.LanPaint_KSampler().sample(patcher, seed, c["steps"], c["cfg"], c["sampler"], c["scheduler"],
-                                                  POS, NEG, {"samples": y, "noise_mask": mask}, 1.0, c["n"],
-                                                  c["mode"], "", N.IMAGE_MODE)
+            torch.cuda.manual_seed(900 + k)     # the generator state a node without a noise image starts from
+            if c["window"] is None:
+                (out,) = N.LanPaint_KSampler().sample(patcher, seed, c["steps"], c["cfg"], c["sampler"],
+                                                      c["scheduler"], POS, NEG, latent, c["denoise"], c["n"],
+                                                      c["mode"], "", N.IMAGE_MODE)
+            else:
+                (out,) = N.LanPaint_KSamplerAdvanced().sample(
+                    patcher, "enable" if c["add_noise"] else "disable", seed, c["steps"], c["cfg"], c["sampler"],
+                    c["scheduler"], POS, NEG, latent, start, end, "enable" if leftover else "disable", c["n"],
+                    c["lam"], c["step_size"], c["mode"], "", N.IMAGE_MODE)
             return out["samples"]
         if k in (0, c["calls"] - 1):
             got, kernels = _sub_kernels(call)
@@ -201,7 +243,11 @@ def test_ksampler_job_matches_fp64(case, cuda_device, monkeypatch):
         offset = gen.get_offset()
         got_steps = list(store)
 
-        noise = minicomfy.prepare_noise(y, seed)      # ComfyUI's CPU noise image; re-seeds every generator like the node
+        torch.cuda.manual_seed(900 + k)
+        if c["add_noise"]:
+            noise = minicomfy.prepare_noise(y, seed)  # ComfyUI's CPU noise image; re-seeds every generator like the node
+        else:
+            noise = torch.zeros(shape)
         yd = y.to(dev, torch.float64)
         dm = _full(mask, shape).to(dev, torch.float64)
         want_steps = []
@@ -215,6 +261,281 @@ def test_ksampler_job_matches_fp64(case, cuda_device, monkeypatch):
         assert modes == c["modes"], modes
     else:
         assert modes[0] == "eager" and all(m in ("job", "steps") for m in modes[1:]), modes
+    N._ENGINES.clear()
+
+
+def _patcher(net, dev, model_type="EPS", shift=1.0, channels=4, opts=None):
+    base = minicomfy.BaseModel(net, model_type=getattr(minicomfy.ModelType, model_type), latent_channels=channels,
+                               shift=shift)
+    patcher = minicomfy.ModelPatcher(base, dev)
+    if opts is not None:
+        patcher.model_options["lanpaint_b200"] = dict(opts)
+    return base, patcher
+
+
+def test_custom_advanced_flux_job_matches_fp64(cuda_device, monkeypatch):
+    """LanPaint_SamplerCustomAdvanced (a GUIDER and a NOISE object) on a Flux latent, simple schedule: both outputs,
+    `output` and `denoised_output` (the last step's denoised latent), against the fp64 job."""
+    minicomfy.install()
+    from lanpaint_b200 import comfy_nodes as N
+    N._ENGINES.clear()
+    dev, case, shape = cuda_device, "custom-adv-flux", (1, 16, 128, 128)
+    base, patcher = _patcher(mixing_denoiser, dev, "FLUX", 1.15, shape[1], {"deferred_max_ms": 1e9})
+    store = []
+    monkeypatch.setattr(sys.modules["latent_preview"], "prepare_callback", _recorder(store))
+    sig = minicomfy.KSampler(patcher, 20, dev, "euler", "simple").sigmas
+    hp = O.Hyper(n_steps=5, lam=6.0, step_size=0.25, min_step_frac=1.0, flow=True)
+    g = torch.Generator().manual_seed(31)
+    y, mask = torch.randn(shape, generator=g), _mask("rand", shape, g)
+    gen = _generator(dev)
+    modes = []
+    for k in range(4):
+        if k == 3:
+            y, mask = torch.randn(shape, generator=g), _mask("rand", shape, g)
+        noise = torch.randn(shape, generator=g)
+        store.clear()
+        guider = minicomfy.CFGGuider(patcher)
+        guider.set_conds(POS, NEG)
+        guider.set_cfg(3.5)
+
+        def call():
+            torch.cuda.manual_seed(700 + k)
+            out, den = N.LanPaint_SamplerCustomAdvanced().sample(
+                FixedNoise(50 + k, noise), guider, minicomfy.ksampler("euler"), sig,
+                {"samples": y, "noise_mask": mask}, 5, 6.0, 0.25, "Prompt First", "")
+            return out["samples"], den["samples"]
+        if k in (0, 3):
+            (got, got_den), kernels = _sub_kernels(call)
+            _assert_torch_tma(f"{case} call {k}", kernels, True)
+        else:
+            got, got_den = call()
+        modes.append(N.LAST_RUN["mode"])
+        torch.cuda.synchronize()
+        offset = gen.get_offset()
+        got_steps = list(store)
+        torch.cuda.manual_seed(700 + k)
+        want_steps = []
+        model = J.Guider(mixing_denoiser, O.FlowSampling(), 3.5, 1.0)       # Flux: cfg_BIG = 1
+        dm = _full(mask, shape).to(dev, torch.float64)
+        want = J.job(J.SAMPLERS["euler"], model, y.to(dev, torch.float64), noise.to(dev, torch.float64), dm, sig, hp,
+                     max_denoise=J.max_denoise(base.model_sampling, sig[0]), callback=lambda i, d: want_steps.append(d))
+        assert gen.get_offset() == offset, f"{case} call {k}: generator offset differs from the reference's"
+        _check(case, f"call {k} out", got, want)
+        _check(case, f"call {k} denoised_output", got_den, want_steps[-1])
+        _check_steps(case, f"call {k}", got_steps, want_steps, y.to(dev), (_full(mask, shape) <= 0.5).to(dev))
+    assert modes[0] == "eager" and all(m in ("job", "steps") for m in modes[1:]) and N.LAST_RUN["fused"], modes
+    N._ENGINES.clear()
+
+
+def test_av_pack_job_matches_fp64(cuda_device, monkeypatch):
+    """A MiniMax-H3 audio-video flat pack of 4.7 M elements through the patched CFGGuider.outer_sample with
+    `latent_shapes`: the per-sigma route with the row split, the audio rows' own schedule and target correction at
+    every outer step.  No TMA sub-step kernel runs under a row split."""
+    minicomfy.install()
+    from lanpaint_b200 import comfy_nodes as N
+    N._ENGINES.clear()
+    monkeypatch.setattr(N, "time_shift_sigma", av_shift_sigma)
+    monkeypatch.setattr(N, "time_shift_slope", av_shift_slope)
+    dev, case = cuda_device, "av-pack-4.7M"
+    n_video, n_audio, sv, sa = 245760, 49152, 3.0, 1.5
+    shape = (1, 16, n_video + n_audio)
+
+    def net(x, sigma, cond):
+        return mixing_denoiser(x, sigma, cond)
+    net.sigma_shift_video, net.sigma_shift_audio = sv, sa
+    base, patcher = _patcher(net, dev, "FLOW", 3.0, shape[1])
+    N._set_hyper(patcher, num_steps=5, cfg=3.5, prompt_mode="Image First")
+    sig = minicomfy.KSampler(patcher, 12, dev, "euler", "simple").sigmas
+    hp = O.Hyper(n_steps=5, min_step_frac=1.0, flow=True)
+    g = torch.Generator().manual_seed(17)
+    gen = _generator(dev)
+    for k in range(4):
+        if k in (0, 3):
+            y = torch.randn(shape, generator=g)
+            mask = (torch.rand(shape, generator=g) < 0.5).float()
+        noise = torch.randn(shape, generator=g)
+        guider = minicomfy.CFGGuider(patcher)
+        guider.set_conds(POS, NEG)
+        guider.set_cfg(3.5)
+
+        def call():
+            torch.cuda.manual_seed(800 + k)
+            with N.override_sample_function():
+                return type(guider).outer_sample(guider, noise, y, minicomfy.ksampler("euler"), sig, denoise_mask=mask,
+                                                 seed=2, latent_shapes=[(1, n_video), (1, n_audio)])
+        if k in (0, 3):
+            got, kernels = _lp_kernels(call)
+            _assert_family(f"{case} call {k}", kernels, "substep_torchvec_kernel")
+            assert not any("tma" in n for n in kernels), (case, sorted(kernels))
+        else:
+            got = call()
+        assert N.LAST_RUN["fused"] is False and N.LAST_RUN["mode"] is None, N.LAST_RUN
+        torch.cuda.synchronize()
+        offset = gen.get_offset()
+        torch.cuda.manual_seed(800 + k)
+        model = J.Guider(mixing_denoiser, O.FlowSampling(), 3.5, 3.5)
+        want = J.job(J.SAMPLERS["euler"], model, y.to(dev, torch.float64), noise.to(dev, torch.float64),
+                     mask.to(dev, torch.float64), sig, hp, max_denoise=J.max_denoise(base.model_sampling, sig[0]),
+                     audio=J.av_audio(n_video, sv, sa))
+        assert gen.get_offset() == offset, f"{case} call {k}: generator offset differs from the reference's"
+        _check(case, f"call {k} out", got, want)
+    N._ENGINES.clear()
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# inner early stop: the GPU's stop points replayed by the fp64 job, every check restated in fp64
+# ---------------------------------------------------------------------------------------------------------------
+ES_THRESHOLD = 0.7   # chosen once for the fixed seeds below: 3 outer steps of each job stop mid-loop, and every
+ES_MARGIN = 0.01     # distance lands >= 8 % from its threshold in an fp32 CPU run of the same jobs (other draws)
+
+
+def _ring(known):
+    """Free sites with a known 4-neighbour, over the last two axes."""
+    near = torch.zeros_like(known)
+    near[..., 1:, :] |= known[..., :-1, :]
+    near[..., :-1, :] |= known[..., 1:, :]
+    near[..., :, 1:] |= known[..., :, :-1]
+    near[..., :, :-1] |= known[..., :, 1:]
+    return (~known) & near
+
+
+def _stop_checks(rec, free, ring, threshold_eff, patience_eff):
+    """The stopper of one outer step restated in fp64 over the fp64 job's states: lp_stop_stats_f32's two sums
+    (free elements, ring elements) of squared differences -- of the VP states around sub-step 0 for the first check,
+    of consecutive x0 estimates after that, and of the x0 estimate and its anchor for the drift guard -- each divided
+    by its element count as earlystop.py does; then the patience counter.  Returns one dict per check."""
+    w_in, w_ring = float(free.sum()), float(ring.sum())
+
+    def stats(a, b):
+        d2 = (a - b) ** 2
+        return float((d2 * free).sum()) / (w_in + 1e-12), float((d2 * ring).sum()) / (w_ring + 1e-12)
+    out, anchor, counter = [], None, 0
+    for j, x0 in enumerate(rec["x0"]):
+        if j == 0:
+            d_in, d_ring = stats(rec["x"][1], rec["x"][0])[0], None
+            dist = d_in
+        else:
+            d_in, d_ring = stats(x0, rec["x0"][j - 1])
+            dist = max(d_in, d_ring)
+        tested, d_drift = [dist], None
+        if dist <= threshold_eff:
+            if anchor is None:
+                anchor = x0
+            else:
+                d_drift = max(stats(x0, anchor))
+                dist = max(dist, d_drift)
+                tested.append(dist)
+        else:
+            anchor = None
+        if dist <= threshold_eff:
+            counter += 1
+        else:
+            counter, anchor = 0, None
+        out.append(dict(dist_inpaint=d_in, dist_ring=d_ring, dist_drift=d_drift, dist=dist, patience_counter=counter,
+                        stopped=counter >= patience_eff, tested=tested))
+    return out
+
+
+def test_early_stop_job_matches_fp64(cuda_device, monkeypatch):
+    """LanPaint_KSampler with the semantic stop on: the un-fused sub-step loop (x0 side output, lp_advance_f32,
+    lp_stop_stats_f32, a decision after every sub-step).  The fp64 job stops where the GPU run's trace stopped; every
+    recorded distance must equal its fp64 restatement, every decision must be the one the fp64 distances give, and
+    every distance must clear the threshold by a margin, so that no decision rests on round-off."""
+    minicomfy.install()
+    from lanpaint_b200 import comfy_nodes as N
+    N._ENGINES.clear()
+    dev, case, shape, n = cuda_device, "early-stop", (8, 4, 128, 128), 10
+    base, patcher = _patcher(mixing_denoiser, dev)
+    trace = []
+    patcher.model_options["lanpaint_semantic_stop"] = {"threshold": ES_THRESHOLD, "patience": 1}
+    patcher.model_options["lanpaint_semantic_trace"] = trace
+    store = []
+    monkeypatch.setattr(sys.modules["latent_preview"], "prepare_callback", _recorder(store))
+    sig = J.ksampler_sigmas(patcher, 20, "euler", "karras")
+    hp = O.Hyper(n_steps=n, min_step_frac=1.0)
+    g = torch.Generator().manual_seed(57)
+    gen = _generator(dev)
+    for k in range(2):
+        mid_loop = 0
+        y, mask = torch.randn(shape, generator=g), _mask("rand", shape, g)
+        seed = 60 + k
+        store.clear()
+        trace.clear()
+
+        def call():
+            (out,) = N.LanPaint_KSampler().sample(patcher, seed, 20, 5.0, "euler", "karras", POS, NEG,
+                                                  {"samples": y, "noise_mask": mask}, 1.0, n, "Image First", "",
+                                                  N.IMAGE_MODE)
+            return out["samples"]
+        got, kernels = _lp_kernels(call)
+        _assert_family(f"{case} call {k}", kernels, "substep_torchvec_kernel")
+        assert any(n_.startswith("advance_") for n_ in kernels) and any(n_.startswith("stop_stats") for n_ in kernels)
+        assert N.LAST_RUN["fused"] is False and N.LAST_RUN["mode"] is None, N.LAST_RUN
+        torch.cuda.synchronize()
+        offset = gen.get_offset()
+        got_steps = list(store)
+        # the GPU's checks, one group per outer step that ran sub-steps
+        groups = []
+        for t in trace:
+            if t["inner_step"] == 1:
+                groups.append([])
+            groups[-1].append(t)
+        recs = []
+
+        class Recorder(J.Guider):
+            """Keeps the latest network input: sub-step 0's is the VE-space state the first check compares with."""
+
+            def __call__(self, x, sigma, model_options=None, seed=None):
+                self.last_x = x
+                return super().__call__(x, sigma, model_options, seed)
+        model = Recorder(mixing_denoiser, O.VESampling(), 5.0, 5.0)
+
+        def on_substep(call):
+            rec = {"x": [], "x0": []}
+            s = float(sig[call])             # Euler: one wrapper call per outer step
+
+            def hook(i, x_t, state):
+                if i == 0:
+                    rec["group"] = groups[len(recs)]
+                    recs.append(rec)
+                    rec["x"].append(model.last_x / (1.0 + s * s) ** 0.5)   # x_t = x / sqrt(1 + VE^2)
+                rec["x"].append(x_t)
+                rec["x0"].append(state.x0)
+                return i + 1 == len(rec["group"]) and rec["group"][-1]["stopped"]
+            return hook
+        noise = minicomfy.prepare_noise(y, seed)
+        want_steps = []
+        dm = _full(mask, shape).to(dev, torch.float64)
+        want = J.job(J.SAMPLERS["euler"], model, y.to(dev, torch.float64), noise.to(dev, torch.float64), dm, sig, hp,
+                     max_denoise=J.max_denoise(base.model_sampling, sig[0]), callback=lambda i, d: want_steps.append(d),
+                     on_substep=on_substep)
+        assert len(recs) == len(groups), (len(recs), len(groups))
+        assert gen.get_offset() == offset, f"{case} call {k}: generator offset differs from the reference's"
+        _check(case, f"call {k} out", got, want)
+        _check_steps(case, f"call {k}", got_steps, want_steps, y.to(dev), (_full(mask, shape) <= 0.5).to(dev))
+
+        known = (mask.to(dev) <= 0.5).expand(shape)
+        free, ring = (~known).double(), _ring(mask.to(dev) <= 0.5).expand(shape).double()
+        for s_i, rec in enumerate(recs):
+            grp = rec["group"]
+            assert len(rec["x0"]) == len(grp)
+            abt = float(grp[0]["abt"])
+            assert abs(grp[0]["threshold_eff"] - ES_THRESHOLD * min(1.0, 4 * abt * (1 - abt))) <= 1e-6 * ES_THRESHOLD
+            want_checks = _stop_checks(rec, free, ring, grp[0]["threshold_eff"], grp[0]["patience_eff"])
+            for t, w in zip(grp, want_checks):
+                where = f"{case} call {k} outer step {s_i} check {t['inner_step']}"
+                for key in ("dist_inpaint", "dist_ring", "dist_drift", "dist"):
+                    if w[key] is None:
+                        assert t[key] is None, (where, key, t[key])
+                    else:
+                        assert abs(t[key] - w[key]) <= 1e-4 * abs(w[key]), (where, key, t[key], w[key])
+                assert (t["patience_counter"], t["stopped"]) == (w["patience_counter"], w["stopped"]), (where, t, w)
+                for d in w["tested"]:
+                    assert abs(d / t["threshold_eff"] - 1.0) >= ES_MARGIN, (where, "decision within the margin", d)
+            s32 = sig[s_i:s_i + 1].float()
+            if grp[-1]["stopped"] and len(grp) < O.inner_steps_for(s32, sig.float(), O.times_from_sigma(s32, False).abt, n):
+                mid_loop += 1
+        assert mid_loop >= 2, f"{case} call {k}: only {mid_loop} outer steps stopped mid-loop"
     N._ENGINES.clear()
 
 
