@@ -331,6 +331,32 @@ int lp_boundary_known(const lp_heads* model_out, const float* y, const float* no
                       const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
                       const lp_dims* dims, lp_stream_t stream);
 
+/* One outer step of k-diffusion's sample_euler_ancestral, as the host precomputes it (get_ancestral_step in Python
+ * doubles, then one rounding to fp32 per field). */
+typedef struct lp_ancestral {
+  float sigma;    /* sigma_from: d = (x - out) / sigma */
+  float down;     /* (float)(sigma_down - sigma_from), the difference taken in double */
+  float s_noise;  /* multiplies the draw first ... */
+  float sigma_up; /* ... then this (0 when eta == 0: the draw is still taken) */
+} lp_ancestral;
+
+/* The boundary of an outer step of a host-owned ANCESTRAL Euler loop in ONE pass: lp_boundary_known with the Euler
+ * update replaced by sample_euler_ancestral's, the sampler's own torch.randn_like(x) drawn inside the kernel:
+ *   d   = model_out->combine ? b + (a - b)*cfg : a
+ *   out = mask ? y : d                                                  written when out != NULL
+ *   x   = x + ((x - out) / sigma) * down
+ *   x   = x + (xi * s_noise) * sigma_up                                 when rng != NULL; xi = the launch's draw
+ *   x   = mask ? rep_noise*noise + rep_y*y : x  (row of next_table)     when next_table != NULL
+ * Every operation of the update is the single correctly rounded fp32 operation the eager sampler issues (sub, div,
+ * mul, add; never contracted), so x equals the un-fused route's bit for bit.  The sampler draws exactly when
+ * sigma_to > 0, also when eta == 0 makes sigma_up zero: the caller passes rng exactly then (draw0 / tape0 only).
+ * rng == NULL: no draw, no stream position consumed.  known may be NULL (dense y / noise / mask).  With
+ * LP_RNG_TORCH an HBM-bound launch takes a TMA-staged kernel of the torch-stream sub-step's work-group form; every
+ * other launch takes an LDG kernel.  Results do not depend on which. */
+int lp_boundary_ancestral(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                          const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
+                          const lp_rng* rng, const float* next_table, const lp_dims* dims, lp_stream_t stream);
+
 /* Final denoise of an outer step straight from raw cond / uncond predictions:
  *   out = mask ? y : uncond + (cond - uncond)*cfg ;  if x_inout != NULL: x = x + (x - out)*euler_coef. */
 int lp_epilogue_cfg_f32(const float* cond, const float* uncond, float cfg, const float* y, const uint8_t* mask,

@@ -389,6 +389,8 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         step: the whole sampler loop is run by `runner.GraphedJob` -- host-computed schedule, Euler update and
         next replace step fused into the step-boundary kernel, CUDA graphs (one per job, or one per outer step
         with ComfyUI's callback between them when the job is long enough to watch) cached across sample() calls;
+        with the option "fused_ancestral" the same holds for euler_ancestral, whose step and randn_like draw
+        run inside lp_boundary_ancestral;
       * any other deterministic sampler: the first job records which sigmas the sampler hands the wrapper, then
         k-diffusion's sampler function itself is captured into ONE graph (`runner.SamplerGraphJob`);
       * anything else (samplers that draw their own noise, early stop, AV packs, mask schedules): k-diffusion's own
@@ -434,8 +436,11 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
                      MinStepFrac=getattr(patcher, "LanPaint_MinStepFrac", 1.0))
         early_stop = patcher.LanPaint_EarlyStop
         use_graph = _graphs_enabled(opts)
+        eo = self.extra_options or {}
+        sampler_key = (getattr(self.sampler_function, "__name__", ""), float(eo.get("eta", 1.0)),
+                       float(eo.get("s_noise", 1.0)))
         entry = _ENGINES.lookup(model_wrap, x_init, model_k.sigmas_host, hyper, early_stop, max_denoise, opts,
-                                model_options, callback is not None) if use_graph else None
+                                model_options, callback is not None, sampler=sampler_key) if use_graph else None
         engine = entry.engine if entry is not None else None
         if engine is None:
             engine = LanPaint(model_k.inner_model, EarlyStopHook=model_options.get("lanpaint_semantic_hook", None),
@@ -458,10 +463,15 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             timing[0].record()
 
         samples = None
-        if opts.get("fused_sampler", True) and KSAMPLER._fused_euler_ok(self, model_k, denoise_mask, model_options, engine):
+        ancestral = None
+        if opts.get("fused_ancestral", False) and KSAMPLER._fused_ancestral_ok(self, model_k, denoise_mask, model_options,
+                                                                                engine):
+            ancestral = sampler_key[1:]
+        if opts.get("fused_sampler", True) and (ancestral is not None or KSAMPLER._fused_euler_ok(
+                self, model_k, denoise_mask, model_options, engine)):
             samples = KSAMPLER._fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options,
                                         extra_args.get("seed"), is_flux or is_flow, early_stop, callback, total_steps,
-                                        use_graph, opts)
+                                        use_graph, opts, ancestral)
         sg_ok = False
         if samples is None and use_graph and entry is not None and opts.get("sampler_graph", True):
             sg_ok = KSAMPLER._sampler_graph_ok(self, model_k, denoise_mask, model_options, engine, entry)
@@ -525,8 +535,27 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         sig = model_k.sigmas_host
         return len(sig) >= 2 and all(v > 0.0 for v in sig[:-1])
 
+    def _fused_ancestral_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
+        """True when k-diffusion's sample_euler_ancestral around the per-sigma wrapper is the host-owned loop of
+        runner.GraphedJob(sampler="euler_ancestral"): the exclusions of `_fused_euler_ok`, and the sampler's noise
+        drawn from the global generator (the default noise sampler of the stand-in and of the reference fixtures)."""
+        if getattr(self.sampler_function, "__name__", "") != "sample_euler_ancestral":
+            return False
+        if set(self.extra_options or {}) - {"eta", "s_noise"}:
+            return False
+        if denoise_mask is None or model_k.audio_indicator is not None:
+            return False
+        if "denoise_mask_function" in model_options or model_options.get("callback") is not None:
+            return False
+        if float(engine.early_stop_threshold or 0.0) > 0.0 or isinstance(model_options.get("lanpaint_semantic_stop"), dict):
+            return False
+        if engine.rng not in ("torch", "philox"):
+            return False
+        sig = model_k.sigmas_host
+        return len(sig) >= 2 and all(v > 0.0 for v in sig[:-1])
+
     def _fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options, seed, flow,
-                     early_stop, callback, total_steps, use_graph, opts):
+                     early_stop, callback, total_steps, use_graph, opts, ancestral=None):
         from .runner import GraphedJob, HostSchedule
         if not x_init.is_cuda:
             raise RuntimeError("lanpaint_b200 needs the latent on a CUDA device: there is no CPU or eager fallback")
@@ -537,8 +566,10 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         if job is None:
             sched = HostSchedule(model_k.sigmas_host, B, engine.n_steps, flow, early_stop, engine.min_step_frac)
             try:
+                sampler = {} if ancestral is None else dict(sampler="euler_ancestral", eta=ancestral[0],
+                                                            s_noise=ancestral[1])
                 job = GraphedJob(engine, sched, tuple(x_init.shape), x_init.device, flow=flow, external_init=True,
-                                 first_replace_noop=False)
+                                 first_replace_noop=False, **sampler)
             except ValueError:     # noise_scaling is not a linear form: the per-sigma wrapper calls it instead
                 return None
             if entry is not None:
@@ -714,14 +745,16 @@ class _EngineEntry:
 class _EngineCache:
     """A few recently used (engine, GraphedJob) pairs keyed by everything a captured graph bakes in: the
     ModelPatcher, the conditioning objects, both guidance scales, latent shape and device, the sigma schedule,
-    every hyper-parameter, the model_options the network reads, whether a callback wants the denoised latent.
+    every hyper-parameter, the model_options the network reads, whether a callback wants the denoised latent,
+    the sampler function with its eta / s_noise.
     The entry keeps the objects named by id() alive, so an id in the key can never be recycled."""
 
     def __init__(self, capacity: int = 4):
         self.capacity = capacity
         self.entries = {}
 
-    def lookup(self, model_wrap, x, sigmas_host, hyper, early_stop, max_denoise, opts, model_options, has_callback):
+    def lookup(self, model_wrap, x, sigmas_host, hyper, early_stop, max_denoise, opts, model_options, has_callback,
+               sampler=None):
         from .engine import options_fingerprint
         conds = getattr(model_wrap, "original_conds", None) or getattr(model_wrap, "conds", {}) or {}
         pos, neg = conds.get("positive"), conds.get("negative")
@@ -730,7 +763,7 @@ class _EngineCache:
                float(model_wrap.cfg_BIG),
                str(x.device), tuple(x.shape), str(x.dtype), tuple(sigmas_host), tuple(sorted(hyper.items())),
                early_stop, bool(max_denoise), options_fingerprint(opts), options_fingerprint(net_opts),
-               bool(has_callback))
+               bool(has_callback), sampler)   # sampler: (function name, eta, s_noise): entry.job runs that loop only
         entry = self.entries.pop(key, None)
         weights = _weights_fingerprint(model_wrap)
         if entry is not None and entry.weights != weights:

@@ -2,6 +2,8 @@
 //   prologue_kernel     replace step + change of variables              lanpaint.py:85-99
 //   boundary_kernel     final paste [+ CFG combine] [+ k-diffusion Euler update] [+ next replace step]
 //                       lanpaint.py:151-157, sample_euler, lanpaint.py:85-94     (LDG and TMA-staged variants)
+//   boundary_ancestral_kernel / boundary_ancestral_torch_tma_kernel
+//                       the same boundary for k-diffusion's sample_euler_ancestral, its randn_like drawn in-kernel
 //   advance_kernel      one un-fused advance_time_overdamped             lanpaint.py:232-254
 //   stop_stats_kernel   early-stop masked reductions                     earlystop.py:32-55,238-313
 #include "lp_common.cuh"
@@ -273,9 +275,9 @@ int boundary_dispatch(const BoundaryArgs& p, bool v4, int dtype, cudaStream_t s)
   return check_launch();
 }
 
-static int boundary_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
-                         const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
-                         const lp_dims* dims, lp_stream_t stream) {
+// what every boundary entry point rejects, before any CUDA call
+static int boundary_check(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                          const lp_known* known, const float* x_inout, const float* out, const float* next_table) {
   if (!mo || !mo->a || !y || !mask) return LP_ERR_INVALID;
   if (known && (!known->words || !known->y || (next_table && !known->noise))) return LP_ERR_INVALID;
   if (!x_inout && !out) return LP_ERR_INVALID;
@@ -283,21 +285,494 @@ static int boundary_impl(const lp_heads* mo, const float* y, const float* noise,
   const int dtype = mo->dtype;
   if (dtype != LP_DTYPE_F32 && dtype != LP_DTYPE_BF16 && dtype != LP_DTYPE_F16) return LP_ERR_INVALID;
   if (mo->combine && (dtype != LP_DTYPE_F32 || !mo->b || mo->b == mo->a)) return LP_ERR_INVALID;
-  BoundaryArgs p;
-  if (int rc = make_geometry(dims, p.g)) return rc;
-  if (p.g.total == 0) return LP_OK;
+  return LP_OK;
+}
+
+// the operands of a checked call whose geometry p.g is made
+static void boundary_args(BoundaryArgs& p, const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                          const lp_known* known, float* x_inout, float* out, float euler_coef,
+                          const float* next_table) {
   p.a = mo->a; p.b = mo->combine ? mo->b : nullptr; p.y = y; p.noise = noise; p.mask = mask; p.x = x_inout; p.out = out;
   p.kwords = known ? known->words : nullptr; p.yk = known ? known->y : nullptr; p.nk = known ? known->noise : nullptr;
   p.next_table = next_table; p.cfg = mo->cfg; p.coef = euler_coef; p.combine = mo->combine != 0;
   p.l2 = l2_handoff(p.g.total);
-  const bool v4 = geometry_vec4(p.g, mask) && head_aligned(p.a, dtype) && (!p.b || head_aligned(p.b, dtype)) &&
-                  aligned16(y) && (!noise || aligned16(noise)) && (!x_inout || aligned16(x_inout)) &&
-                  (!out || aligned16(out));
+}
+
+static bool boundary_vec4(const BoundaryArgs& p, int dtype) {
+  return geometry_vec4(p.g, p.mask) && head_aligned(p.a, dtype) && (!p.b || head_aligned(p.b, dtype)) &&
+         aligned16(p.y) && (!p.noise || aligned16(p.noise)) && (!p.x || aligned16(p.x)) &&
+         (!p.out || aligned16(p.out));
+}
+
+static int boundary_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                         const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
+                         const lp_dims* dims, lp_stream_t stream) {
+  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
+  BoundaryArgs p;
+  if (int rc = make_geometry(dims, p.g)) return rc;
+  if (p.g.total == 0) return LP_OK;
+  boundary_args(p, mo, y, noise, mask, known, x_inout, out, euler_coef, next_table);
+  const int dtype = mo->dtype;
+  const bool v4 = boundary_vec4(p, dtype);
   cudaStream_t s = (cudaStream_t)stream;
   switch (dtype) {
     case LP_DTYPE_F32: return boundary_dispatch<float>(p, v4, dtype, s);
     case LP_DTYPE_BF16: return boundary_dispatch<__nv_bfloat16>(p, v4, dtype, s);
     default: return boundary_dispatch<__half>(p, v4, dtype, s);
+  }
+}
+
+// ---- the boundary of an outer step of a host-owned ancestral Euler loop ----------------------------------------
+// k-diffusion's sample_euler_ancestral issues, after the wrapper call, sub, div, mul, add, randn_like, mul, mul, add
+// as eight eager kernels; lp_boundary_ancestral does them in the boundary's one pass, each as the same correctly
+// rounded fp32 operation, and draws the sampler's randn_like itself.
+constexpr int kRngNone = -1;  // no rng: sigma_to == 0, the sampler takes no draw
+
+struct AncestralArgs {
+  BoundaryArgs b;  // x is never NULL; coef is unused
+  lp_ancestral st;
+  const float* tape0;
+  const uint64_t* rng_state;
+  uint64_t seed, draw0;
+  uint32_t torch_T;  // threads of torch's randn grid (LP_RNG_TORCH)
+};
+
+// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; x += ((x - o) / sigma) down ;
+// x += (xi s_noise) sigma_up ; x = known ? rn n + ry y : x
+__device__ __forceinline__ void ancestral_element(float a, float b, float y, float nz, bool known, float& x, float& o,
+                                                  bool combine, float cfg, const lp_ancestral& st, bool draw, float xi,
+                                                  bool next, float rn, float ry) {
+  const float d = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
+  o = known ? y : d;
+  x = __fadd_rn(x, __fmul_rn(__fdiv_rn(__fsub_rn(x, o), st.sigma), st.down));
+  if (draw) x = __fadd_rn(x, __fmul_rn(__fmul_rn(xi, st.s_noise), st.sigma_up));
+  if (next) x = known ? fmaf(rn, nz, ry * y) : x;  // rounds as prologue_kernel does
+}
+
+// one N-wide vector: the operand loads of boundary_kernel, x always updated
+template <int N, typename H, bool kPk>
+__device__ __forceinline__ void ancestral_vector(const AncestralArgs& q, uint32_t i, const float (&xi)[N], bool draw) {
+  const BoundaryArgs& p = q.b;
+  const uint64_t dead = l2_policy_dead(p.l2);
+  uint32_t row, mi;
+  locate(p.g, i, row, mi);
+  const bool next = p.next_table != nullptr;
+  float av[N], bv[N], yv[N], xv[N], nv[N], ov[N];
+  bool known[N];
+  uint32_t kb = 0, kidx = 0;
+  if constexpr (kPk) {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
+    if constexpr (N == 4) {
+      known_quad(w, i, kb, kidx);
+    } else {
+      kb = (w.x >> (i & 31u)) & 1u;
+      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
+    }
+#pragma unroll
+    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
+  } else {
+    load_m<N>(p.mask, mi, known);
+  }
+  bool any_known = false, any_free = false;
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    any_known |= known[j];
+    any_free |= !known[j];
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = 0.f;
+  if constexpr (kPk) {
+    if constexpr (N == 4) {
+      gather_known4<false>(p.yk, kb, kidx, yv);
+    } else {
+      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
+    }
+  } else {
+    load_f_ro<N>(p.y, i, yv);
+  }
+  if (any_free) {
+    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
+    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
+  }
+  if (any_free || !next) load_f<N>(p.x, i, xv);
+  float rn = 0.f, ry = 0.f;
+  if (next) {
+    if constexpr (kPk) {
+      if constexpr (N == 4) {
+        gather_known4<false>(p.nk, kb, kidx, nv);
+      } else {
+        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
+      }
+    } else {
+      if (any_known) load_f_ro<N>(p.noise, i, nv);
+    }
+    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
+    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j)
+    ancestral_element(av[j], bv[j], yv[j], nv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st, draw, xi[j], next,
+                      rn, ry);
+  if (p.out) store_f<N>(p.out, i, ov, dead);
+  store_f<N>(p.x, i, xv);
+}
+
+// LDG form: small or ragged launches, and the TAPE / PHILOX streams.  LP_RNG_TORCH maps threads onto torch's own
+// randn grid: N == 4 as substep_torchvec_kernel does (thread (t, k) draws call k of subsequence t, a quad transposes
+// its normals into four consecutive elements), N == 1 as advance_torch_kernel does.
+template <int N, typename H, bool kPk, int kRng>
+__global__ void __launch_bounds__(kBlock) boundary_ancestral_kernel(const AncestralArgs q) {
+  pdl_prologue();
+  const uint32_t total = q.b.g.total;
+  if constexpr (kRng == LP_RNG_TORCH) {
+    uint64_t seed = q.seed, o0 = q.draw0;
+    if (q.rng_state) {
+      seed = q.rng_state[0];
+      o0 += q.rng_state[1];
+    }
+    const uint32_t T = q.torch_T;
+    const uint32_t t = blockIdx.x * kBlock + threadIdx.x;  // torch thread == Philox subsequence
+    if constexpr (N == 4) {
+      const uint32_t k = blockIdx.y, l = t & 3u;
+      const float4 n = torch_normal4(seed, o0, t, k);
+      float xi[4] = {n.x, n.y, n.z, n.w};
+      quad_transpose(xi, l);
+      const uint64_t e = (uint64_t)(t - l) + (uint64_t)(4u * k + l) * T;  // first of my 4 consecutive elements
+      if (e >= total) return;
+      ancestral_vector<4, H, kPk>(q, (uint32_t)e, xi, true);
+    } else {
+      if (t >= T) return;
+      uint32_t call = 0;
+      for (uint64_t base = t; base < total; base += 4ull * T, ++call) {
+        const float4 n = torch_normal4(seed, o0, t, call);
+#pragma unroll
+        for (int ii = 0; ii < 4; ++ii) {
+          const uint64_t li = base + (uint64_t)ii * T;
+          if (li >= total) break;
+          const float xi[1] = {pick(n, ii)};
+          ancestral_vector<1, H, kPk>(q, (uint32_t)li, xi, true);
+        }
+      }
+    }
+  } else {
+    const uint32_t i = (walk_index(q.b.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+    if (i >= total) return;
+    float xi[N];
+#pragma unroll
+    for (int j = 0; j < N; ++j) xi[j] = 0.f;
+    if constexpr (kRng == LP_RNG_TAPE) {
+      load_f_ro<N>(q.tape0, i, xi);
+    } else if constexpr (kRng == LP_RNG_PHILOX) {
+      uint64_t seed = q.seed, d0 = q.draw0;
+      if (q.rng_state) {
+        seed = q.rng_state[0];
+        d0 += q.rng_state[1];
+      }
+      const float4 n = philox_normal4(seed, d0, i >> 2);
+      if constexpr (N == 4) {
+        xi[0] = n.x; xi[1 % N] = n.y; xi[2 % N] = n.z; xi[3 % N] = n.w;
+      } else {
+        xi[0] = pick(n, i & 3);
+      }
+    }
+    ancestral_vector<N, H, kPk>(q, i, xi, kRng != kRngNone);
+  }
+}
+
+// LP_RNG_TORCH at HBM-bound sizes: the work-group form of substep_torch_tma_kernel (lp_substep.cu).  A group is
+// (Philox call k, block b of kG consecutive subsequences) = four sub-tiles of kG consecutive elements, T apart; a
+// producer warp streams each sub-tile's operand slices into its slot of a four-slot ring (full / empty mbarrier
+// pairs) while the eight consumer warps draw; consumer thread c owns subsequences 4c..4c+3, so its four normals of a
+// plane are one float4 of that plane's sub-tile.  One draw per launch.  kPk: the known bits and the packed y / noise
+// spans (widened to 16-byte bounds) replace the dense y / noise slices and the uint8 mask slices.
+template <typename H, int kG, bool kCombine, bool kNext, bool kPk>
+struct __align__(128) AncestralSlot {
+  H a[kG], b[kCombine ? kG : 8];  // every member starts on a 16-byte boundary (cp.async.bulk destinations)
+  float x[kG];
+  float y[kPk ? kG + 8 : kG];
+  float nz[kNext ? (kPk ? kG + 8 : kG) : 4];
+  uint8_t m[kPk ? 16 : kG];
+  uint2 w[kPk ? kG / 32 : 2];
+};
+
+template <typename H, bool kCombine, bool kNext, bool kPk>
+__global__ void __launch_bounds__(1024 / 4 + 32, 2)
+    boundary_ancestral_torch_tma_kernel(const AncestralArgs q, const uint32_t groups_per_call, const uint32_t n_groups) {
+  constexpr int kG = 1024, kConsumers = kG / 4;
+  using Slot = AncestralSlot<H, kG, kCombine, kNext, kPk>;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ __align__(8) uint64_t full[4], empty[4];
+  Slot* slot = reinterpret_cast<Slot*>(smem_raw);
+  pdl_prologue();
+  const BoundaryArgs& p = q.b;
+  const uint32_t T = q.torch_T, total = p.g.total;
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      mbar_init(&full[j], 1);
+      mbar_init(&empty[j], kConsumers);
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  // first element / length of sub-tile j of group (k, b); a sub-tile past the end of the tensor is empty
+  auto subtile = [&](uint32_t k, uint32_t b, int j, uint32_t& e0, uint32_t& len) {
+    const uint64_t e = (uint64_t)(4u * k + (uint32_t)j) * T + (uint64_t)b * kG;
+    if (e >= total) {
+      e0 = 0;
+      len = 0;
+    } else {
+      e0 = (uint32_t)e;
+      len = total - e0 < (uint32_t)kG ? total - e0 : (uint32_t)kG;
+    }
+  };
+
+  if (warp == kConsumers / 32) {  // ---------------- producer ----------------
+    if (lane == 0) {
+      const H* ap = static_cast<const H*>(p.a);
+      const H* bp = static_cast<const H*>(p.b);
+      const uint64_t dead = l2_policy_dead(p.l2);
+      uint32_t it = 0;
+      for (uint32_t step = blockIdx.x; step < n_groups; step += gridDim.x, ++it) {
+        const uint32_t grp = walk_index(p.l2, step, n_groups);  // the consumers map `step` the same way
+        const uint32_t k = grp / groups_per_call, b = grp - k * groups_per_call;
+        uint32_t lo[4] = {0u, 0u, 0u, 0u}, hi[4] = {0u, 0u, 0u, 0u};
+        if constexpr (kPk) {  // the packed spans of the group, read before the first slot wait, which hides them
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            uint32_t e0, len;
+            subtile(k, b, j, e0, len);
+            if (len) {
+              lo[j] = __ldg(p.kwords + 2u * (e0 >> 5) + 1u);
+              hi[j] = __ldg(p.kwords + 2u * ((e0 + len + 31u) >> 5) + 1u);
+            }
+          }
+        }
+#pragma unroll 1
+        for (int j = 0; j < 4; ++j) {
+          mbar_wait_relaxed(&empty[j], (it & 1u) ^ 1u);  // drained by the consumers (passes at once the first time)
+          uint32_t e0, len;
+          subtile(k, b, j, e0, len);
+          const uint32_t fb = len * 4u, hb = len * (uint32_t)sizeof(H);
+          const uint32_t heads = hb * (kCombine ? 2u : 1u);
+          Slot& t = slot[j];
+          if constexpr (kPk) {
+            const uint32_t nw = (((len + 31u) >> 5) + 1u) & ~1u;  // whole words, an even number: 16-byte multiple
+            const uint32_t ylo = (j == 0 ? lo[0] : j == 1 ? lo[1] : j == 2 ? lo[2] : lo[3]) & ~3u;
+            const uint32_t yhi = ((j == 0 ? hi[0] : j == 1 ? hi[1] : j == 2 ? hi[2] : hi[3]) + 3u) & ~3u;
+            const uint32_t yb = (yhi - ylo) * 4u;
+            // an empty sub-tile still completes its phase: expect 0 bytes
+            mbar_expect_tx(&full[j], len ? fb + heads + yb * (kNext ? 2u : 1u) + nw * 8u : 0u);
+            if (len == 0) continue;
+            tma_load_1d(t.a, ap + e0, hb, &full[j], dead);
+            if (kCombine) tma_load_1d(t.b, bp + e0, hb, &full[j], dead);
+            tma_load_1d(t.x, p.x + e0, fb, &full[j]);
+            if (yb) tma_load_1d(t.y, p.yk + ylo, yb, &full[j]);
+            if (kNext && yb) tma_load_1d(t.nz, p.nk + ylo, yb, &full[j]);
+            tma_load_1d(t.w, p.kwords + 2u * (e0 >> 5), nw * 8u, &full[j]);
+          } else {
+            mbar_expect_tx(&full[j], fb * (kNext ? 3u : 2u) + heads + len);
+            if (len == 0) continue;
+            tma_load_1d(t.a, ap + e0, hb, &full[j], dead);
+            if (kCombine) tma_load_1d(t.b, bp + e0, hb, &full[j], dead);
+            tma_load_1d(t.x, p.x + e0, fb, &full[j]);
+            tma_load_1d(t.y, p.y + e0, fb, &full[j]);
+            if (kNext) tma_load_1d(t.nz, p.noise + e0, fb, &full[j]);
+            // the mask is indexed per (row, channel): one slice per channel segment the sub-tile touches
+            uint32_t e = e0, off = 0, rem = len;
+            while (rem) {
+              const uint32_t row = p.g.per_row.div(e);
+              const uint32_t r = e - row * p.g.per_row.d;
+              const uint32_t ch = p.g.spatial.div(r);
+              const uint32_t s = r - ch * p.g.spatial.d;
+              const uint32_t seg = rem < p.g.spatial.d - s ? rem : p.g.spatial.d - s;
+              tma_load_1d(t.m + off, p.mask + row * p.g.mask_row_stride + ch * p.g.mask_channel_stride + s, seg,
+                          &full[j]);
+              e += seg;
+              off += seg;
+              rem -= seg;
+            }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ---------------- consumers ----------------
+  uint64_t seed = q.seed, o0 = q.draw0;
+  if (q.rng_state) {
+    seed = q.rng_state[0];
+    o0 += q.rng_state[1];
+  }
+  const uint32_t tid = threadIdx.x;  // vector index inside every sub-tile
+  // one sub-tile's vector of this thread: slot -> registers, slot released, update, stores
+  auto vector = [&](int j, uint32_t i, const float (&xi)[4]) {
+    const Slot& t = slot[j];
+    float a[4], b[4] = {0.f, 0.f, 0.f, 0.f}, y[4], nz[4] = {0.f, 0.f, 0.f, 0.f}, o[4];
+    uint32_t kb;
+    lds_head4<H>(t.a, tid, a);
+    if (kCombine) lds_head4<H>(t.b, tid, b);
+    const float4 xv = reinterpret_cast<const float4*>(t.x)[tid];
+    if constexpr (kPk) {
+      uint32_t idx;
+      known_quad(t.w[tid >> 3], 4u * tid, kb, idx);
+      idx -= t.w[0].y & ~3u;  // the spans start at the first word's base, rounded down
+      gather_known4<true>(t.y, kb, idx, y);
+      if (kNext) gather_known4<true>(t.nz, kb, idx, nz);
+    } else {
+      const float4 yv = reinterpret_cast<const float4*>(t.y)[tid];
+      const uchar4 mv = reinterpret_cast<const uchar4*>(t.m)[tid];
+      y[0] = yv.x; y[1] = yv.y; y[2] = yv.z; y[3] = yv.w;
+      kb = (mv.x != 0 ? 1u : 0u) | (mv.y != 0 ? 2u : 0u) | (mv.z != 0 ? 4u : 0u) | (mv.w != 0 ? 8u : 0u);
+      if (kNext) {
+        const float4 nv = reinterpret_cast<const float4*>(t.nz)[tid];
+        nz[0] = nv.x; nz[1] = nv.y; nz[2] = nv.z; nz[3] = nv.w;
+      }
+    }
+    mbar_arrive(&empty[j]);  // this thread's reads of slot j are in registers: let it refill
+    float x[4] = {xv.x, xv.y, xv.z, xv.w};
+    float rn = 0.f, ry = 0.f;
+    if (kNext) {
+      const uint32_t row = p.g.per_row.div(i);
+      rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
+      ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      ancestral_element(a[e], b[e], y[e], nz[e], ((kb >> e) & 1u) != 0, x[e], o[e], kCombine, p.cfg, q.st, true, xi[e],
+                        kNext, rn, ry);
+    if (p.out) st_f4(p.out + i, make_float4(o[0], o[1], o[2], o[3]), l2_policy_dead(p.l2));
+    *reinterpret_cast<float4*>(p.x + i) = make_float4(x[0], x[1], x[2], x[3]);
+  };
+  uint32_t it = 0;
+  for (uint32_t step = blockIdx.x; step < n_groups; step += gridDim.x, ++it) {
+    const uint32_t grp = walk_index(p.l2, step, n_groups);
+    const uint32_t k = grp / groups_per_call, b = grp - k * groups_per_call;
+    const uint32_t t0 = b * kG + 4u * tid;  // my four Philox subsequences (torch threads)
+    uint4 r[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) r[i] = torch_philox(seed, o0, t0 + i, k);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // curand_normal4: planes 0,1 <- (x,y), planes 2,3 <- (z,w)
+      float2 n[4];
+#pragma unroll
+      for (int i = 0; i < 4; i += 2)
+        box_muller_curand_x2(h ? r[i].z : r[i].x, h ? r[i].w : r[i].y, h ? r[i + 1].z : r[i + 1].x,
+                             h ? r[i + 1].w : r[i + 1].y, n[i], n[i + 1]);
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        const int j = 2 * h + jj;
+        const float xi[4] = {jj ? n[0].y : n[0].x, jj ? n[1].y : n[1].x, jj ? n[2].y : n[2].x, jj ? n[3].y : n[3].x};
+        mbar_wait(&full[j], it & 1u);
+        uint32_t e0, len;
+        subtile(k, b, j, e0, len);
+        if (4u * tid < len) vector(j, e0 + 4u * tid, xi);
+        else mbar_arrive(&empty[j]);
+      }
+    }
+  }
+}
+
+template <typename H, bool kCombine, bool kNext, bool kPk>
+int launch_ancestral_tma_cfg(const AncestralArgs& q, uint32_t calls, cudaStream_t s) {
+  const int dev = current_device();
+  const size_t smem = sizeof(AncestralSlot<H, 1024, kCombine, kNext, kPk>) * 4;
+  const uint32_t groups_per_call = q.torch_T / 1024, n_groups = calls * groups_per_call;
+  unsigned grid = (unsigned)device_info(dev).sms * 2u;
+  if (grid > n_groups) grid = n_groups;
+  static bool configured[kMaxDevices] = {};  // per instantiation of this launcher
+  ensure_dynamic_smem(boundary_ancestral_torch_tma_kernel<H, kCombine, kNext, kPk>, smem, dev, configured);
+  launch_kernel_ex(boundary_ancestral_torch_tma_kernel<H, kCombine, kNext, kPk>, dim3(grid), dim3(1024 / 4 + 32), smem,
+                   s, q, groups_per_call, n_groups);
+  return check_launch();
+}
+
+template <typename H, bool kCombine>
+int launch_ancestral_tma(const AncestralArgs& q, bool packed, uint32_t calls, cudaStream_t s) {
+  const bool next = q.b.next_table != nullptr;
+  if (packed) {
+    return next ? launch_ancestral_tma_cfg<H, kCombine, true, true>(q, calls, s)
+                : launch_ancestral_tma_cfg<H, kCombine, false, true>(q, calls, s);
+  }
+  return next ? launch_ancestral_tma_cfg<H, kCombine, true, false>(q, calls, s)
+              : launch_ancestral_tma_cfg<H, kCombine, false, false>(q, calls, s);
+}
+
+template <int N, typename H, int kRng>
+void launch_ancestral_ldg(const AncestralArgs& q, dim3 grid, cudaStream_t s) {
+  if (q.b.kwords) launch_kernel(boundary_ancestral_kernel<N, H, true, kRng>, grid, s, q);
+  else launch_kernel(boundary_ancestral_kernel<N, H, false, kRng>, grid, s, q);
+}
+
+template <typename H>
+int ancestral_dispatch(AncestralArgs& q, int mode, bool v4, cudaStream_t s) {
+  const BoundaryArgs& p = q.b;
+  const dim3 flat(v4 ? blocks_for(p.g.total / 4) : blocks_for(p.g.total));
+  if (mode == LP_RNG_TORCH) {
+    int64_t grid = 0;
+    if (int rc = torch_grid(p.g.total, -1, &grid, nullptr)) return rc;
+    q.torch_T = (uint32_t)(grid * 256);
+    const uint64_t calls = ((uint64_t)p.g.total + 4ull * q.torch_T - 1) / (4ull * q.torch_T);
+    // the torch-stream TMA sub-step's eligibility (lp_substep.cu)
+    const bool tma = v4 && g_opt_tma != 0 && geometry_tma(p.g, p.mask) && p.g.total >= (uint32_t)g_opt_tma_min &&
+                     aligned16(p.a) && (!p.combine || aligned16(p.b)) && aligned16(p.y) &&
+                     (!p.next_table || aligned16(p.noise)) && q.torch_T % 1024 == 0 && p.g.spatial.d >= 64 &&
+                     calls <= 0xffffffffull / 4;
+    if (tma) {
+      const bool packed = p.kwords && aligned16(p.kwords) && aligned16(p.yk) && (!p.next_table || aligned16(p.nk));
+      if constexpr (sizeof(H) == 4) {  // the CFG combine needs fp32 heads
+        if (p.combine) return launch_ancestral_tma<H, true>(q, packed, (uint32_t)calls, s);
+      }
+      return launch_ancestral_tma<H, false>(q, packed, (uint32_t)calls, s);
+    }
+    if (v4 && calls <= 65535) launch_ancestral_ldg<4, H, LP_RNG_TORCH>(q, dim3((unsigned)grid, (unsigned)calls), s);
+    else launch_ancestral_ldg<1, H, LP_RNG_TORCH>(q, dim3((unsigned)grid), s);
+  } else if (mode == LP_RNG_TAPE) {
+    if (v4 && aligned16(q.tape0)) launch_ancestral_ldg<4, H, LP_RNG_TAPE>(q, flat, s);
+    else launch_ancestral_ldg<1, H, LP_RNG_TAPE>(q, dim3(blocks_for(p.g.total)), s);
+  } else if (mode == LP_RNG_PHILOX) {
+    if (v4) launch_ancestral_ldg<4, H, LP_RNG_PHILOX>(q, flat, s);
+    else launch_ancestral_ldg<1, H, LP_RNG_PHILOX>(q, flat, s);
+  } else {
+    if (v4) launch_ancestral_ldg<4, H, kRngNone>(q, flat, s);
+    else launch_ancestral_ldg<1, H, kRngNone>(q, flat, s);
+  }
+  return check_launch();
+}
+
+static int boundary_ancestral_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                                   const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
+                                   const lp_rng* rng, const float* next_table, const lp_dims* dims,
+                                   lp_stream_t stream) {
+  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
+  if (!x_inout || !step || !(step->sigma > 0.f)) return LP_ERR_INVALID;
+  if (!rng && step->sigma_up != 0.f) return LP_ERR_INVALID;
+  int mode = kRngNone;
+  if (rng) {
+    mode = rng->mode;
+    if (mode != LP_RNG_TAPE && mode != LP_RNG_PHILOX && mode != LP_RNG_TORCH) return LP_ERR_INVALID;
+    if (mode == LP_RNG_TAPE && !rng->tape0) return LP_ERR_INVALID;
+  }
+  AncestralArgs q;
+  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  if (q.b.g.total == 0) return LP_OK;
+  boundary_args(q.b, mo, y, noise, mask, known, x_inout, out, 0.f, next_table);
+  q.st = *step;
+  q.tape0 = rng ? rng->tape0 : nullptr;
+  q.rng_state = rng ? rng->state : nullptr;
+  q.seed = rng ? rng->seed : 0;
+  q.draw0 = rng ? rng->draw0 : 0;
+  q.torch_T = 0;
+  const int dtype = mo->dtype;
+  const bool v4 = boundary_vec4(q.b, dtype);
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (dtype) {
+    case LP_DTYPE_F32: return ancestral_dispatch<float>(q, mode, v4, s);
+    case LP_DTYPE_BF16: return ancestral_dispatch<__nv_bfloat16>(q, mode, v4, s);
+    default: return ancestral_dispatch<__half>(q, mode, v4, s);
   }
 }
 
@@ -465,6 +940,13 @@ extern "C" int lp_boundary_known(const lp_heads* model_out, const float* y, cons
                                  const float* next_table, const lp_dims* dims, lp_stream_t stream) {
   if (!known) return LP_ERR_INVALID;
   return boundary_impl(model_out, y, noise, mask, known, x_inout, out, euler_coef, next_table, dims, stream);
+}
+
+extern "C" int lp_boundary_ancestral(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                                     const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
+                                     const lp_rng* rng, const float* next_table, const lp_dims* dims,
+                                     lp_stream_t stream) {
+  return boundary_ancestral_impl(model_out, y, noise, mask, known, x_inout, out, step, rng, next_table, dims, stream);
 }
 
 extern "C" int lp_epilogue_f32(const float* model_out, const float* y, const uint8_t* mask, float* out,

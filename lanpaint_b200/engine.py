@@ -531,7 +531,7 @@ class LanPaint:
     # ---- the launch sequence of one outer step (shared by the eager path and graph capture) ----
     def _launch_sequence(self, xm, y, nz, pm, dims, tab, t_model, sigma_dev, cbuf, out, active, plan, call_scaling,
                          model_options, seed, stopper, rng_state, euler_coef=None, skip_prologue=False,
-                         next_table=None, current_times=None):
+                         next_table=None, current_times=None, ancestral=None):
         lib = _native.load()
         dev = xm.device
         stream = _P(_stream_ptr(dev))
@@ -640,6 +640,20 @@ class LanPaint:
         else:
             mo, _ = self.unpack_model_output(out_heads)
             hd, keep = _heads(mo, None, xm)
+        if ancestral is not None:
+            # host-owned sample_euler_ancestral loop: (lp_ancestral, whether the sampler draws at this step).  Its
+            # randn_like comes after the step's Langevin draws, so its position is taken here, not earlier
+            step, draws = ancestral
+            r = plan.rng_struct(1, rng_state) if draws else None
+            rc = lib.lp_boundary_ancestral(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
+                                           C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
+                                           _P(xm.data_ptr()), _P(_ptr(out)), C.byref(step),
+                                           C.byref(r) if r is not None else None,
+                                           _P(next_table.data_ptr()) if next_table is not None else None,
+                                           C.byref(dims), stream)
+            _native.check(rc, "lp_boundary_ancestral")
+            self.launches += 1
+            return done
         fused_next = next_table is not None and euler_coef is not None
         if kn is not None and (kn.noise is not None or not fused_next):
             rc = lib.lp_boundary_known(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()) if fused_next else None,

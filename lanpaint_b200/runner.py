@@ -20,7 +20,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _native
-from .schedule import effective_inner_steps, times_from_sigma
+from .schedule import ancestral_step, effective_inner_steps, times_from_sigma
 
 
 class VESampling:
@@ -164,6 +164,38 @@ def euler_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask,
     return x
 
 
+def _sampler_draw(engine, x: torch.Tensor) -> torch.Tensor:
+    """The sampler's own `torch.randn_like(x)` on the engine's stream: the global generator itself for "torch", the
+    next whole-tensor draw index of the same generator for "philox" (lp_fill_normal_f32)."""
+    if engine.rng == "torch":
+        return torch.randn_like(x)
+    from .engine import _DrawPlan
+    plan = _DrawPlan(engine.rng, x, 1)
+    xi = torch.empty_like(x)
+    r = plan.rng_struct(1)
+    rc = _native.load().lp_fill_normal_f32(C.c_void_p(xi.data_ptr()), xi.numel(), C.byref(r),
+                                           C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream))
+    _native.check(rc, "lp_fill_normal_f32")
+    plan.finish()
+    return xi
+
+
+def euler_ancestral_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask, sched: HostSchedule,
+                            eta: float = 1.0, s_noise: float = 1.0) -> torch.Tensor:
+    """`euler_inpaint` with k-diffusion's sample_euler_ancestral as the sampler: the un-fused definition of
+    GraphedJob(sampler="euler_ancestral"), eager torch ops and the sampler's own draw after every wrapper call."""
+    sampling = engine.inner_model.inner_model.model_sampling
+    x = sampling.noise_scaling(sched.sigmas[0].to(latent_image.device), noise, latent_image)
+    for st in sched.steps:
+        denoised = engine(x, latent_image, noise, st.sigma_t, mask, st.times, None, 0, n_steps=st.n_inner)
+        s_down, s_up = ancestral_step(st.sigma, st.sigma_next, eta)
+        d = (x - denoised) / st.sigma_t.to(x.device).reshape((-1,) + (1,) * (x.ndim - 1))
+        x = x + d * (s_down - st.sigma)
+        if st.sigma_next > 0:
+            x = x + _sampler_draw(engine, x) * s_noise * s_up
+    return x
+
+
 def time_steady_substep(engine, latent_image: torch.Tensor, mask, sigma: float, launches: int = 53,
                         repeats: int = 20, flow: bool = False, rotate: int = 3):
     """Roofline probe: `launches` steady fused sub-step launches (flags = FUSE_NEXT, the kernel that
@@ -253,10 +285,13 @@ class GraphedJob:
 
     def __init__(self, engine, sched: HostSchedule, shape, device, flow: bool = False, fused_euler: bool = True,
                  l2_persist: bool = False, model_options=None, seed=0, external_init: bool = False,
-                 first_replace_noop=None):
+                 first_replace_noop=None, sampler: str = "euler", eta: float = 1.0, s_noise: float = 1.0):
         import numpy as np
         from .engine import _DrawPlan
-        self.fused_euler = fused_euler   # Euler update inside lp_epilogue_euler_f32 instead of two torch kernels
+        if sampler not in ("euler", "euler_ancestral"):
+            raise ValueError(f"GraphedJob owns the loops of 'euler' and 'euler_ancestral', not {sampler!r}")
+        self.sampler = sampler
+        self.fused_euler = fused_euler   # the sampler's update inside the step-boundary kernel instead of torch kernels
         # optional persisting-L2 window over the clean latent (re-read by every launch).  Off by default: the
         # set-aside takes L2 away from absorbing the sub-step's writes, which can cost more than the y hits give back
         self.l2_persist = l2_persist
@@ -289,9 +324,19 @@ class GraphedJob:
         # draws consumed before outer step i (1 for sub-step 0, 2 for each later one): lets every outer step be
         # captured on its own against ONE {seed, base} block that is refreshed once per job
         merged = engine.rng == "philox" and engine.merge_noise   # a fused launch then draws ONE normal, not two
+        # euler_ancestral: one lp_ancestral per outer step, and the sampler's randn_like -- taken whenever
+        # sigma_next > 0, whatever eta makes of sigma_up -- as one more draw after the step's Langevin draws
+        self.ancestral = None
+        if sampler == "euler_ancestral":
+            self.ancestral = []
+            for st in sched.steps:
+                s_down, s_up = ancestral_step(st.sigma, st.sigma_next, eta)
+                self.ancestral.append((_native.Ancestral(st.sigma, s_down - st.sigma, s_noise, s_up),
+                                       st.sigma_next > 0))
         self.draws_before = [0]
-        for n in self.active:
-            self.draws_before.append(self.draws_before[-1] + (0 if n <= 0 else (n if merged else 2 * n - 1)))
+        for i, n in enumerate(self.active):
+            own = 1 if (self.ancestral is not None and self.ancestral[i][1]) else 0
+            self.draws_before.append(self.draws_before[-1] + (0 if n <= 0 else (n if merged else 2 * n - 1)) + own)
         self.tables = torch.from_numpy(np.stack(tabs)).to(dev)
         self.t_model = torch.from_numpy(np.stack(tms).astype(np.float32)).to(dev)
         self.sigma = torch.from_numpy(np.stack(sgs).astype(np.float32)).to(dev)
@@ -332,6 +377,7 @@ class GraphedJob:
         eng = self.engine
         st = self.sched.steps[i]
         coef = (st.sigma_next - st.sigma) / st.sigma
+        anc = self.ancestral[i] if self.ancestral is not None else None
         last = i + 1 == len(self.sched.steps)
         plan.used = self.draws_before[i]
         out = self.out if (want_out or not self.fused_euler) else None
@@ -339,11 +385,27 @@ class GraphedJob:
             out = self.outs[i]
         eng._launch_sequence(self.x, self.y, self.noise, self.mask, self._dims, self.tables[i], self.t_model[i],
                              self.sigma[i], self.c, out, self.active[i], plan, False, self.model_options, self.seed,
-                             None, self.rng_state.data_ptr(), euler_coef=coef if self.fused_euler else None,
+                             None, self.rng_state.data_ptr(),
+                             euler_coef=coef if (self.fused_euler and anc is None) else None,
                              skip_prologue=(self.fused_euler and i > 0) or (i == 0 and self.first_replace_noop),
-                             next_table=self.tables[i + 1] if (self.fused_euler and not last) else None)
-        if not self.fused_euler:     # from this step's denoised latent, wherever it was written
+                             next_table=self.tables[i + 1] if (self.fused_euler and not last) else None,
+                             ancestral=anc if self.fused_euler else None)
+        if self.fused_euler:
+            return
+        # un-fused: from this step's denoised latent, wherever it was written
+        if anc is None:
             self.x.add_(self.x - out, alpha=coef)
+            return
+        step, draws = anc
+        d = (self.x - out) / self.sigma[i].reshape((-1,) + (1,) * (self.x.ndim - 1))
+        self.x.add_(d * step.down)
+        if draws:   # torch.randn_like's values at the plan's position, by a capturable launch
+            xi = torch.empty_like(self.x)
+            r = plan.rng_struct(1, self.rng_state.data_ptr())
+            rc = _native.load().lp_fill_normal_f32(C.c_void_p(xi.data_ptr()), xi.numel(), C.byref(r),
+                                                   C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            _native.check(rc, "lp_fill_normal_f32")
+            self.x.add_(xi * step.s_noise * step.sigma_up)
 
     def _body(self, plan, want_out):
         if not self.external_init:

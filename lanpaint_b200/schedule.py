@@ -59,6 +59,16 @@ def effective_inner_steps(n_steps: int, sigmas_host: Sequence[float], sigma_mean
     return min_step_frac_effective_steps(n_steps, abt_frac, min_frac)
 
 
+def ancestral_step(sigma_from: float, sigma_to: float, eta: float = 1.0):
+    """(sigma_down, sigma_up) of one step of k-diffusion's sample_euler_ancestral (get_ancestral_step), in Python
+    doubles with the sampler's own expression, operation for operation: the fused loop rounds what the sampler
+    rounds."""
+    s_from, s_to = float(sigma_from), float(sigma_to)
+    s_up = min(s_to, eta * (s_to ** 2 * (s_from ** 2 - s_to ** 2) / s_from ** 2) ** 0.5) if s_to > 0 else 0.0
+    s_down = (s_to ** 2 - s_up ** 2) ** 0.5
+    return s_down, s_up
+
+
 @dataclass
 class Hyper:
     step_size: float
