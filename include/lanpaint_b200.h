@@ -31,6 +31,9 @@ extern "C" {
 #endif
 
 #define LP_ABI_VERSION 5
+/* Backward-compatible additions within LP_ABI_VERSION: 1 = LP_HEADS_DEAD (a dtype bit every earlier library
+ * rejected with LP_ERR_INVALID, so no earlier caller can have set it). */
+#define LP_ABI_MINOR 1
 #define LP_TABLE_STRIDE 32 /* floats per table row (one 128-byte line), layout below */
 
 typedef void* lp_stream_t; /* a cudaStream_t / CUstream */
@@ -118,6 +121,15 @@ typedef struct lp_rng {
  * separate .float() pass (6 B/element read + 8 B/element written per head pair). */
 typedef enum lp_dtype { LP_DTYPE_F32 = 0, LP_DTYPE_BF16 = 1, LP_DTYPE_F16 = 2 } lp_dtype;
 
+/* lp_heads.dtype may carry this bit next to the lp_dtype: nothing reads a or b after the launch.  The HBM-bound
+ * update kernels (the TMA-staged sub-steps, the LDG step boundary, the TMA-staged ancestral boundary) then drop
+ * every 128-byte line of the heads they have finished reading from the L2 without writing it back
+ * (discard.global.L2): a network's output is still dirty in L2 when the update that consumes it starts, and its
+ * write-back is HBM traffic nothing needs.  Afterwards the heads' memory holds undefined values until it is written
+ * again.  A launch ignores the bit unless both heads start on a 128-byte boundary and no output of the launch
+ * overlaps them; option "discard_heads" 0 ignores it everywhere.  Results do not depend on it. */
+enum { LP_HEADS_DEAD = 0x100 };
+
 /* The model's prediction(s) for one call, as the kernels consume them (src/LanPaint/lanpaint.py:34-43,
  * 159-171; src/LanPaint/nodes.py:161-175):
  *   combine == 0   a = x0, b = x0_BIG (NULL or == a: the two heads alias)
@@ -127,7 +139,7 @@ typedef enum lp_dtype { LP_DTYPE_F32 = 0, LP_DTYPE_BF16 = 1, LP_DTYPE_F16 = 2 } 
 typedef struct lp_heads {
   const void* a;
   const void* b;
-  int32_t dtype;   /* lp_dtype of a and b */
+  int32_t dtype;   /* lp_dtype of a and b, optionally | LP_HEADS_DEAD */
   int32_t combine;
   float cfg, cfg_big;
 } lp_heads;
@@ -149,7 +161,8 @@ int lp_last_cuda_error(void); /* cudaError_t of the last failed launch on this t
  *   "l2_handoff"   bits, for measurement: 1 the TMA sub-steps and the step-boundary kernels walk their launch
  *                  tail-first, 2 evict-first L2 policy on the heads, C and the boundary's output (default 3);
  *                  launches of fewer than 2^20 elements, whose job stays in L2, use neither.  Results do not
- *                  depend on it. */
+ *                  depend on it.
+ *   "discard_heads" 1|0  honour LP_HEADS_DEAD (default 1; 0 for measurement) */
 int lp_set_option(const char* name, int value);
 
 /* Host-only self test of the index arithmetic the kernels rely on (the multiply-shift division that

@@ -17,6 +17,7 @@ TABLE_STRIDE = 32
 
 RNG_TAPE, RNG_PHILOX, RNG_TORCH = 0, 1, 2
 DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2
+HEADS_DEAD = 0x100  # LP_HEADS_DEAD: or-ed into Heads.dtype when nothing reads the heads after the launch
 T_INVS = 2  # LP_T_INVS
 SUBSTEP_FIRST, SUBSTEP_FUSE_NEXT, SUBSTEP_STORE_C, SUBSTEP_MERGE_NOISE = 1, 2, 4, 8
 

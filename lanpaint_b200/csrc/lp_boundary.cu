@@ -52,6 +52,8 @@ struct BoundaryArgs {
   float cfg, coef;
   int combine;
   int l2;          // kL2* bits of this launch (l2_handoff)
+  int discard;     // the heads are dead after this launch (LP_HEADS_DEAD, heads_discard): the LDG boundary and the
+                   // TMA-staged ancestral boundary drop their L2 lines once read
   Geometry g;
 };
 
@@ -136,6 +138,16 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
                      ry);
   if (p.out) store_f<N>(p.out, i, ov, dead);
   if (euler) store_f<N>(p.x, i, xv);
+  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
+    if (p.discard) {
+      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
+      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
+        __syncwarp();           // every lane's head loads are used
+        discard_line<H>(p.a, i, end);
+        if (p.b) discard_line<H>(p.b, i, end);
+      }
+    }
+  }
 }
 
 // TMA-staged persistent variant for HBM-bound sizes (fused Euler loop: x is always updated).  Same tile walk and
@@ -282,7 +294,7 @@ static int boundary_check(const lp_heads* mo, const float* y, const float* noise
   if (known && (!known->words || !known->y || (next_table && !known->noise))) return LP_ERR_INVALID;
   if (!x_inout && !out) return LP_ERR_INVALID;
   if (next_table && (!noise || !x_inout)) return LP_ERR_INVALID;
-  const int dtype = mo->dtype;
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
   if (dtype != LP_DTYPE_F32 && dtype != LP_DTYPE_BF16 && dtype != LP_DTYPE_F16) return LP_ERR_INVALID;
   if (mo->combine && (dtype != LP_DTYPE_F32 || !mo->b || mo->b == mo->a)) return LP_ERR_INVALID;
   return LP_OK;
@@ -296,6 +308,7 @@ static void boundary_args(BoundaryArgs& p, const lp_heads* mo, const float* y, c
   p.kwords = known ? known->words : nullptr; p.yk = known ? known->y : nullptr; p.nk = known ? known->noise : nullptr;
   p.next_table = next_table; p.cfg = mo->cfg; p.coef = euler_coef; p.combine = mo->combine != 0;
   p.l2 = l2_handoff(p.g.total);
+  p.discard = heads_discard(mo, p.b, p.g.total, {x_inout, out});
 }
 
 static bool boundary_vec4(const BoundaryArgs& p, int dtype) {
@@ -312,7 +325,7 @@ static int boundary_impl(const lp_heads* mo, const float* y, const float* noise,
   if (int rc = make_geometry(dims, p.g)) return rc;
   if (p.g.total == 0) return LP_OK;
   boundary_args(p, mo, y, noise, mask, known, x_inout, out, euler_coef, next_table);
-  const int dtype = mo->dtype;
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
   const bool v4 = boundary_vec4(p, dtype);
   cudaStream_t s = (cudaStream_t)stream;
   switch (dtype) {
@@ -633,6 +646,10 @@ __global__ void __launch_bounds__(1024 / 4 + 32, 2)
       }
     }
     mbar_arrive(&empty[j]);  // this thread's reads of slot j are in registers: let it refill
+    if (p.discard) {  // sub-tiles start on multiples of kG elements: a line below `total` lies in slot j
+      discard_line<H>(p.a, i, total);
+      if (kCombine) discard_line<H>(p.b, i, total);
+    }
     float x[4] = {xv.x, xv.y, xv.z, xv.w};
     float rn = 0.f, ry = 0.f;
     if (kNext) {
@@ -766,7 +783,7 @@ static int boundary_ancestral_impl(const lp_heads* mo, const float* y, const flo
   q.seed = rng ? rng->seed : 0;
   q.draw0 = rng ? rng->draw0 : 0;
   q.torch_T = 0;
-  const int dtype = mo->dtype;
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
   const bool v4 = boundary_vec4(q.b, dtype);
   cudaStream_t s = (cudaStream_t)stream;
   switch (dtype) {

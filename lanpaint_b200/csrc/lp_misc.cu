@@ -29,6 +29,7 @@ int g_opt_l2_handoff = [] {
   const char* e = getenv("LANPAINT_B200_L2_HANDOFF");
   return e ? atoi(e) : kL2Default;
 }();
+int g_opt_discard_heads = 1;
 
 int current_device() {
   int dev = 0;
@@ -353,6 +354,7 @@ extern "C" int lp_set_option(const char* name, int value) {
   if (eq("tma_min")) { g_opt_tma_min = value; return LP_OK; }
   if (eq("tma_boundary")) { g_opt_tma_boundary = value; return LP_OK; }
   if (eq("l2_handoff")) { g_opt_l2_handoff = value; return LP_OK; }
+  if (eq("discard_heads")) { g_opt_discard_heads = value; return LP_OK; }
   return LP_ERR_INVALID;
 }
 

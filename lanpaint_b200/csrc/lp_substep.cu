@@ -35,6 +35,8 @@ struct SubstepArgs {
   int store_c;       // write C even when the next half-advance is not fused
   int use_cfg;       // x0/x0b hold raw cond/uncond predictions: combine them here
   int l2;            // kL2* bits of this launch (l2_handoff)
+  int discard;       // the heads are dead after this launch (LP_HEADS_DEAD, heads_discard): the TMA-staged kernels
+                     // drop their L2 lines once the lines are in shared memory
   float cfg, cfg_big;
 };
 
@@ -187,9 +189,9 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) substep_tma_kernel(const S
     tma_load_1d(t.x, a.x + e0, fb, &full[s]);
     tma_load_1d(t.x0, x0p + e0, hb, &full[s], dead);
     if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[s], dead);
-    tma_load_1d(t.y, a.y + e0, fb, &full[s]);
+    tma_load_1d(t.y, a.y + e0, fb, &full[s], dead);
     if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[s], dead);
-    tma_load_1d(t.m, a.mask + mi0, len, &full[s]);
+    tma_load_1d(t.m, a.mask + mi0, len, &full[s], dead);
   };
 
   uint64_t seed = a.seed, d0 = a.draw0, d1 = a.draw1;
@@ -248,6 +250,10 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) substep_tma_kernel(const S
                                                 te[j]);
         *reinterpret_cast<float4*>(a.x + i) = make_float4(x[0], x[1], x[2], x[3]);
         if (kNext || a.store_c) st_f4(a.c + i, make_float4(cn[0], cn[1], cn[2], cn[3]), dead);
+        if (a.discard) {  // the tile's bytes landed in shared memory before the wait above returned
+          discard_line<H>(a.x0, i, e0 + len);
+          if (!aliased) discard_line<H>(a.x0b, i, e0 + len);
+        }
       }
     }
     __syncthreads();  // every thread is done reading stage s
@@ -360,9 +366,9 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
             tma_load_1d(t.x, a.x + e0, fb, &full[j]);
             tma_load_1d(t.x0, x0p + e0, hb, &full[j], dead);
             if (!aliased) tma_load_1d(t.x0b, x0bp + e0, hb, &full[j], dead);
-            if (yb) tma_load_1d(t.y, a.yk + ylo, yb, &full[j]);
+            if (yb) tma_load_1d(t.y, a.yk + ylo, yb, &full[j], dead);
             if (!kFirst) tma_load_1d(t.c, a.c + e0, fb, &full[j], dead);
-            tma_load_1d(t.w, a.kwords + 2u * (e0 >> 5), nw * 8u, &full[j]);
+            tma_load_1d(t.w, a.kwords + 2u * (e0 >> 5), nw * 8u, &full[j], dead);
           } else {
             mbar_expect_tx(&full[j], fb * (2u + (kFirst ? 0u : 1u)) + heads + len);
             if (len == 0) continue;
@@ -455,6 +461,13 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
   // __syncwarp() is no faster, and compute-sanitizer's racecheck cannot follow that form: it reports hazards against
   // the producer's next cp.async.bulk; with per-thread arrives it reports none.)
   auto release = [&](int j) { mbar_arrive(&empty[j]); };
+  // dead heads: sub-tiles start on multiples of kG elements, so a line below `total` lies in the slot just waited for
+  auto drop = [&](uint32_t i) {
+    if (a.discard) {
+      discard_line<H>(a.x0, i, total);
+      if (!aliased) discard_line<H>(a.x0b, i, total);
+    }
+  };
   uint32_t it = 0;
   for (uint32_t step = blockIdx.x; step < tg.n_groups; step += gridDim.x, ++it) {
     const uint32_t grp = walk_index(a.l2, step, tg.n_groups);
@@ -492,13 +505,17 @@ __device__ __forceinline__ void torch_tma_body(const SubstepArgs& a, const Torch
           fetch(slot[j], x, x0, x0b, y, cp, kb);
           release(j);  // this warp's reads of slot j are in registers: let it refill
           finish((4u * k + (uint32_t)j) * T + t0, x, x0, x0b, y, cp, kb, p1, p2, jj);
+          drop((4u * k + (uint32_t)j) * T + t0);
         } else {
           uint32_t e0, len;
           subtile(k, b, j, e0, len);
           const bool active = 4u * tid < len;
           if (active) fetch(slot[j], x, x0, x0b, y, cp, kb);
           release(j);
-          if (active) finish(e0 + 4u * tid, x, x0, x0b, y, cp, kb, p1, p2, jj);
+          if (active) {
+            finish(e0 + 4u * tid, x, x0, x0b, y, cp, kb, p1, p2, jj);
+            drop(e0 + 4u * tid);
+          }
         }
       }
     }
@@ -731,7 +748,7 @@ static int substep_impl(float* x_model, const lp_heads* heads, const float* y, c
   if (known && (!known->words || !known->y)) return LP_ERR_INVALID;
   if (flags & ~(LP_SUBSTEP_FIRST | LP_SUBSTEP_FUSE_NEXT | LP_SUBSTEP_STORE_C | LP_SUBSTEP_MERGE_NOISE))
     return LP_ERR_INVALID;
-  const int dtype = heads->dtype;
+  const int dtype = heads->dtype & ~LP_HEADS_DEAD;
   if (dtype != LP_DTYPE_F32 && dtype != LP_DTYPE_BF16 && dtype != LP_DTYPE_F16) return LP_ERR_INVALID;
   if (heads->combine && (dtype != LP_DTYPE_F32 || !heads->b || heads->b == heads->a)) return LP_ERR_INVALID;
   const bool merge = (flags & LP_SUBSTEP_MERGE_NOISE) != 0;
@@ -753,6 +770,7 @@ static int substep_impl(float* x_model, const lp_heads* heads, const float* y, c
   a.store_c = (flags & LP_SUBSTEP_STORE_C) != 0;
   a.use_cfg = heads->combine != 0; a.cfg = heads->cfg; a.cfg_big = heads->cfg_big;
   a.l2 = l2_handoff(a.g.total);
+  a.discard = heads_discard(heads, x0_big != x0 ? x0_big : nullptr, a.g.total, {x_model, c_state, x_copy, x0e_out});
   cudaStream_t s = (cudaStream_t)stream;
   const bool v4 = geometry_vec4(a.g, mask) && aligned16(x_model) && head_aligned(x0, dtype) &&
                   head_aligned(x0_big, dtype) && aligned16(y) && (!c_state || aligned16(c_state)) &&

@@ -516,22 +516,27 @@ class LanPaint:
         return {"table": torch.from_numpy(table_np).to(device), "t_model": torch.from_numpy(tm_h.copy()).to(device),
                 "sigma": sigma_host.to(device=device, dtype=torch.float32).reshape(shape), "active": int(active)}
 
-    def run_planned(self, x, item, y, nz, pm, dims, cbuf, plan, rng_state, model_options, seed):
+    def run_planned(self, x, item, y, nz, pm, dims, cbuf, plan, rng_state, model_options, seed, discard_heads=False):
         """One wrapper call from a plan_item: no host read-back, no H2D copy, no generator access -- only kernel
-        launches and the model calls, i.e. capturable as part of a larger CUDA graph.  x is rewritten in place."""
+        launches and the model calls, i.e. capturable as part of a larger CUDA graph.  x is rewritten in place.
+        discard_heads: see `_launch_sequence`."""
         if not (x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()):
             raise RuntimeError("planned LanPaint call needs a contiguous fp32 CUDA state tensor")
         self.img_dim_size = x.ndim
         out = torch.empty_like(x)
         done = self._launch_sequence(x, y, nz, pm, dims, item["table"], item["t_model"], item["sigma"], cbuf, out,
-                                     item["active"], plan, False, model_options, seed, None, rng_state)
+                                     item["active"], plan, False, model_options, seed, None, rng_state,
+                                     discard_heads=discard_heads)
         self.substeps_done += done
         return out
 
     # ---- the launch sequence of one outer step (shared by the eager path and graph capture) ----
     def _launch_sequence(self, xm, y, nz, pm, dims, tab, t_model, sigma_dev, cbuf, out, active, plan, call_scaling,
                          model_options, seed, stopper, rng_state, euler_coef=None, skip_prologue=False,
-                         next_table=None, current_times=None, ancestral=None):
+                         next_table=None, current_times=None, ancestral=None, discard_heads=False):
+        """discard_heads: the caller owns the network's outputs and nothing reads them once the update kernel that
+        consumes them has run (`heads_discardable`), so that kernel may drop them from the L2 unwritten
+        (LP_HEADS_DEAD).  Only the fused loop's launches take it; the early-stop loop hands the heads to the stopper."""
         lib = _native.load()
         dev = xm.device
         stream = _P(_stream_ptr(dev))
@@ -559,10 +564,11 @@ class LanPaint:
                 heads = self.inner_model(xm, t_model, model_options=model_options, seed=seed)
                 if isinstance(heads, CfgPair) and stopper is None and heads.cond.dtype == torch.float32 \
                         and heads.uncond.dtype == torch.float32:
-                    hd, keep = _heads(heads.cond, heads.uncond, xm, True, heads.cfg, heads.cfg_big)
+                    hd, keep = _heads(heads.cond, heads.uncond, xm, True, heads.cfg, heads.cfg_big,
+                                      dead=discard_heads)
                 else:
                     h0, h1 = self.unpack_model_output(heads)
-                    hd, keep = _heads(h0, h1, xm)
+                    hd, keep = _heads(h0, h1, xm, dead=discard_heads and stopper is None)
             if stopper is None:
                 # fused: post-model half of sub-step i + pre-model half of sub-step i+1
                 flags = (F.SUBSTEP_FIRST if first else 0) | (F.SUBSTEP_FUSE_NEXT if has_next else 0)
@@ -636,10 +642,11 @@ class LanPaint:
         self.model_calls += 1
         if isinstance(out_heads, CfgPair) and out_heads.cond.dtype == torch.float32 \
                 and out_heads.uncond.dtype == torch.float32:
-            hd, keep = _heads(out_heads.cond, out_heads.uncond, xm, True, out_heads.cfg, out_heads.cfg)
+            hd, keep = _heads(out_heads.cond, out_heads.uncond, xm, True, out_heads.cfg, out_heads.cfg,
+                              dead=discard_heads)
         else:
             mo, _ = self.unpack_model_output(out_heads)
-            hd, keep = _heads(mo, None, xm)
+            hd, keep = _heads(mo, None, xm, dead=discard_heads)
         if ancestral is not None:
             # host-owned sample_euler_ancestral loop: (lp_ancestral, whether the sampler draws at this step).  Its
             # randn_like comes after the step's Langevin draws, so its position is taken here, not earlier
@@ -1006,14 +1013,26 @@ def _as_operand(t: torch.Tensor, like: torch.Tensor) -> torch.Tensor:
 
 
 def _heads(a: torch.Tensor, b: Optional[torch.Tensor], like: torch.Tensor, combine: bool = False, cfg: float = 0.0,
-           cfg_big: float = 0.0):
-    """-> (lp_heads struct, tensors to keep alive).  a / b end up with one common dtype."""
+           cfg_big: float = 0.0, dead: bool = False):
+    """-> (lp_heads struct, tensors to keep alive).  a / b end up with one common dtype.  dead: LP_HEADS_DEAD."""
     a = _as_operand(a, like)
     b = a if (b is None or b is a) else _as_operand(b, like)
     if b.dtype != a.dtype or (combine and a.dtype != torch.float32):
         a, b = a.float(), (a.float() if b is a else b.float())
-    h = _native.Heads(a.data_ptr(), b.data_ptr(), _HEAD_DTYPES[a.dtype], 1 if combine else 0, float(cfg), float(cfg_big))
+    h = _native.Heads(a.data_ptr(), b.data_ptr(), _HEAD_DTYPES[a.dtype] | (_native.HEADS_DEAD if dead else 0),
+                      1 if combine else 0, float(cfg), float(cfg_big))
     return h, (a, b)
+
+
+def heads_discardable(model_options) -> bool:
+    """Whether a job that owns its network calls may let the update kernels discard the network's outputs once read
+    (`_launch_sequence(discard_heads=True)`): not when a user CFG hook has seen them (ComfyUI's sampler_cfg_function
+    / sampler_post_cfg_function receive the raw predictions and may keep them), nor when the network re-reads its
+    own output and says so with the option {"discard_heads": False}."""
+    mo = model_options or {}
+    if not (mo.get("lanpaint_b200") or {}).get("discard_heads", True):
+        return False
+    return "sampler_cfg_function" not in mo and not mo.get("sampler_post_cfg_function")
 
 
 def _probe_noise_scaling(sampling, sigma: float):

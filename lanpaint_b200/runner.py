@@ -383,9 +383,11 @@ class GraphedJob:
         out = self.out if (want_out or not self.fused_euler) else None
         if want_out == "each":      # every outer step keeps its own denoised latent
             out = self.outs[i]
+        from .engine import heads_discardable
+        # the job owns every network call it makes, and the next one overwrites what the last update read
         eng._launch_sequence(self.x, self.y, self.noise, self.mask, self._dims, self.tables[i], self.t_model[i],
                              self.sigma[i], self.c, out, self.active[i], plan, False, self.model_options, self.seed,
-                             None, self.rng_state.data_ptr(),
+                             None, self.rng_state.data_ptr(), discard_heads=heads_discardable(self.model_options),
                              euler_coef=coef if (self.fused_euler and anc is None) else None,
                              skip_prologue=(self.fused_euler and i > 0) or (i == 0 and self.first_replace_noop),
                              next_table=self.tables[i + 1] if (self.fused_euler and not last) else None,
@@ -606,6 +608,7 @@ class SamplerGraphJob:
         self.mask.known = pack_known(self.mask, self.dims, self.y, self.noise, out=self.mask.known)
 
     def _capture(self, model_k, extra_args, want_callbacks):
+        from .engine import heads_discardable
         eng = self.engine
         B = self.shape[0]
         self.items = []
@@ -625,7 +628,7 @@ class SamplerGraphJob:
             item = job.items[state["pos"]]
             state["pos"] += 1
             return eng.run_planned(x, item, job.y, job.noise, job.mask, job.dims, job.c, plan, job.rng_state.data_ptr(),
-                                   model_options, seed)
+                                   model_options, seed, discard_heads=heads_discardable(model_options))
         model_k.planned_call = planned
         self.recorded = []
         k_callback = None
