@@ -32,8 +32,9 @@ extern "C" {
 
 #define LP_ABI_VERSION 5
 /* Backward-compatible additions within LP_ABI_VERSION: 1 = LP_HEADS_DEAD (a dtype bit every earlier library
- * rejected with LP_ERR_INVALID, so no earlier caller can have set it). */
-#define LP_ABI_MINOR 1
+ * rejected with LP_ERR_INVALID, so no earlier caller can have set it); 2 = lp_multistep and
+ * lp_boundary_multistep (a new entry point: nothing an earlier caller binds changes). */
+#define LP_ABI_MINOR 2
 #define LP_TABLE_STRIDE 32 /* floats per table row (one 128-byte line), layout below */
 
 typedef void* lp_stream_t; /* a cudaStream_t / CUstream */
@@ -369,6 +370,32 @@ typedef struct lp_ancestral {
 int lp_boundary_ancestral(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                           const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
                           const lp_rng* rng, const float* next_table, const lp_dims* dims, lp_stream_t stream);
+
+/* One outer step of k-diffusion's sample_dpmpp_2m (DPM-Solver++(2M)), with t = -log(sigma) and h = t_next - t.  The
+ * host evaluates these with the sampler's own torch expressions on the schedule, on the device the sampler runs on,
+ * and reads them back: they are the fp32 scalars the sampler multiplies with. */
+typedef struct lp_multistep {
+  float ratio; /* sigma_fn(t_next) / sigma_fn(t), sigma_fn(t) = exp(-t): 0 on the step to sigma = 0 */
+  float em1;   /* expm1(-h): -1 on the step to sigma = 0 */
+  float c_cur; /* 1 + 1/(2r), r = h_last / h: weight of this step's denoised latent (second-order steps) */
+  float c_old; /* 1/(2r): weight of the previous step's denoised latent (second-order steps) */
+} lp_multistep;
+
+/* The boundary of an outer step of a host-owned DPM-Solver++(2M) loop in ONE pass: lp_boundary_known with the Euler
+ * update replaced by sample_dpmpp_2m's:
+ *   d   = model_out->combine ? b + (a - b)*cfg : a
+ *   out = mask ? y : d                                                  written when out != NULL
+ *   x   = ratio*x - em1*out                                             when old_out == NULL (first order)
+ *   x   = ratio*x - em1*(c_cur*out - c_old*old_out)                     otherwise (second order)
+ *   x   = mask ? rep_noise*noise + rep_y*y : x  (row of next_table)     when next_table != NULL
+ * old_out is the previous step's `out`.  The sampler takes the first-order branch on its first step and on the step
+ * to sigma = 0: the caller passes old_out == NULL exactly then.  Every operation of the update is the single
+ * correctly rounded fp32 operation the eager sampler issues (mul, sub; never contracted), so x equals the un-fused
+ * route's bit for bit.  old_out is read only where the update survives (free positions; known positions too when
+ * next_table == NULL) and must not overlap x_inout or out.  known may be NULL (dense y / noise / mask). */
+int lp_boundary_multistep(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                          const lp_known* known, float* x_inout, float* out, const float* old_out,
+                          const lp_multistep* step, const float* next_table, const lp_dims* dims, lp_stream_t stream);
 
 /* Final denoise of an outer step straight from raw cond / uncond predictions:
  *   out = mask ? y : uncond + (cond - uncond)*cfg ;  if x_inout != NULL: x = x + (x - out)*euler_coef. */

@@ -390,7 +390,8 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         next replace step fused into the step-boundary kernel, CUDA graphs (one per job, or one per outer step
         with ComfyUI's callback between them when the job is long enough to watch) cached across sample() calls;
         with the option "fused_ancestral" the same holds for euler_ancestral, whose step and randn_like draw
-        run inside lp_boundary_ancestral;
+        run inside lp_boundary_ancestral; dpmpp_2m runs there too (on by default), its update and the previous
+        step's denoised latent inside lp_boundary_multistep;
       * any other deterministic sampler: the first job records which sigmas the sampler hands the wrapper, then
         k-diffusion's sampler function itself is captured into ONE graph (`runner.SamplerGraphJob`);
       * anything else (samplers that draw their own noise, early stop, AV packs, mask schedules): k-diffusion's own
@@ -467,11 +468,13 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         if opts.get("fused_ancestral", False) and KSAMPLER._fused_ancestral_ok(self, model_k, denoise_mask, model_options,
                                                                                 engine):
             ancestral = sampler_key[1:]
-        if opts.get("fused_sampler", True) and (ancestral is not None or KSAMPLER._fused_euler_ok(
+        multistep = ancestral is None and KSAMPLER._fused_dpmpp_2m_ok(self, model_k, denoise_mask, model_options,
+                                                                      engine)
+        if opts.get("fused_sampler", True) and (ancestral is not None or multistep or KSAMPLER._fused_euler_ok(
                 self, model_k, denoise_mask, model_options, engine)):
             samples = KSAMPLER._fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options,
                                         extra_args.get("seed"), is_flux or is_flow, early_stop, callback, total_steps,
-                                        use_graph, opts, ancestral)
+                                        use_graph, opts, ancestral, multistep)
         sg_ok = False
         if samples is None and use_graph and entry is not None and opts.get("sampler_graph", True):
             sg_ok = KSAMPLER._sampler_graph_ok(self, model_k, denoise_mask, model_options, engine, entry)
@@ -514,6 +517,21 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         return base.model_sampling.inverse_noise_scaling(sigmas[-1], samples)
 
     # ---- plain Euler: the sampler loop as one launch sequence ---------------------------------------
+    @staticmethod
+    def _fused_loop_ok(model_k, denoise_mask, model_options, engine) -> bool:
+        """What every host-owned loop of runner.GraphedJob needs: an inpainting mask, nothing that runs host code or
+        changes the mask inside an outer step, an in-kernel RNG, every sigma but the last > 0."""
+        if denoise_mask is None or model_k.audio_indicator is not None:
+            return False
+        if "denoise_mask_function" in model_options or model_options.get("callback") is not None:
+            return False
+        if float(engine.early_stop_threshold or 0.0) > 0.0 or isinstance(model_options.get("lanpaint_semantic_stop"), dict):
+            return False
+        if engine.rng not in ("torch", "philox"):
+            return False
+        sig = model_k.sigmas_host
+        return len(sig) >= 2 and all(v > 0.0 for v in sig[:-1])
+
     def _fused_euler_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
         """True when k-diffusion's sample_euler around the per-sigma wrapper is exactly the host-owned loop of
         runner.GraphedJob: default Euler (no churn), an inpainting mask, nothing that runs host code or changes
@@ -524,16 +542,7 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         eo = self.extra_options or {}
         if float(eo.get("s_churn", 0.0) or 0.0) != 0.0 or float(eo.get("s_noise", 1.0) or 1.0) != 1.0:
             return False
-        if denoise_mask is None or model_k.audio_indicator is not None:
-            return False
-        if "denoise_mask_function" in model_options or model_options.get("callback") is not None:
-            return False
-        if float(engine.early_stop_threshold or 0.0) > 0.0 or isinstance(model_options.get("lanpaint_semantic_stop"), dict):
-            return False
-        if engine.rng not in ("torch", "philox"):
-            return False
-        sig = model_k.sigmas_host
-        return len(sig) >= 2 and all(v > 0.0 for v in sig[:-1])
+        return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
 
     def _fused_ancestral_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
         """True when k-diffusion's sample_euler_ancestral around the per-sigma wrapper is the host-owned loop of
@@ -543,19 +552,18 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             return False
         if set(self.extra_options or {}) - {"eta", "s_noise"}:
             return False
-        if denoise_mask is None or model_k.audio_indicator is not None:
+        return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
+
+    def _fused_dpmpp_2m_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
+        """True when k-diffusion's sample_dpmpp_2m around the per-sigma wrapper is the host-owned loop of
+        runner.GraphedJob(sampler="dpmpp_2m"): the sampler without extra options, and the exclusions of
+        `_fused_euler_ok`."""
+        if getattr(self.sampler_function, "__name__", "") != "sample_dpmpp_2m" or self.extra_options:
             return False
-        if "denoise_mask_function" in model_options or model_options.get("callback") is not None:
-            return False
-        if float(engine.early_stop_threshold or 0.0) > 0.0 or isinstance(model_options.get("lanpaint_semantic_stop"), dict):
-            return False
-        if engine.rng not in ("torch", "philox"):
-            return False
-        sig = model_k.sigmas_host
-        return len(sig) >= 2 and all(v > 0.0 for v in sig[:-1])
+        return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
 
     def _fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options, seed, flow,
-                     early_stop, callback, total_steps, use_graph, opts, ancestral=None):
+                     early_stop, callback, total_steps, use_graph, opts, ancestral=None, multistep=False):
         from .runner import GraphedJob, HostSchedule
         if not x_init.is_cuda:
             raise RuntimeError("lanpaint_b200 needs the latent on a CUDA device: there is no CPU or eager fallback")
@@ -568,6 +576,8 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             try:
                 sampler = {} if ancestral is None else dict(sampler="euler_ancestral", eta=ancestral[0],
                                                             s_noise=ancestral[1])
+                if multistep:
+                    sampler = dict(sampler="dpmpp_2m")
                 job = GraphedJob(engine, sched, tuple(x_init.shape), x_init.device, flow=flow, external_init=True,
                                  first_replace_noop=False, **sampler)
             except ValueError:     # noise_scaling is not a linear form: the per-sigma wrapper calls it instead

@@ -4,6 +4,8 @@
 //                       lanpaint.py:151-157, sample_euler, lanpaint.py:85-94     (LDG and TMA-staged variants)
 //   boundary_ancestral_kernel / boundary_ancestral_torch_tma_kernel
 //                       the same boundary for k-diffusion's sample_euler_ancestral, its randn_like drawn in-kernel
+//   boundary_multistep_kernel
+//                       the same boundary for k-diffusion's sample_dpmpp_2m (DPM-Solver++(2M))
 //   advance_kernel      one un-fused advance_time_overdamped             lanpaint.py:232-254
 //   stop_stats_kernel   early-stop masked reductions                     earlystop.py:32-55,238-313
 #include "lp_common.cuh"
@@ -793,6 +795,157 @@ static int boundary_ancestral_impl(const lp_heads* mo, const float* y, const flo
   }
 }
 
+// ---- the boundary of an outer step of a host-owned DPM-Solver++(2M) loop --------------------------------------
+// k-diffusion's sample_dpmpp_2m issues, after the wrapper call, mul, mul, sub (first order) or mul, mul, sub, mul, mul,
+// sub (second order) as eager kernels, with per-step 0-d tensors the host hands in as lp_multistep;
+// lp_boundary_multistep does them in the boundary's one pass, each as the same correctly rounded fp32 operation.
+struct MultistepArgs {
+  BoundaryArgs b;  // x is never NULL; coef is unused
+  lp_multistep st;
+  const float* old;  // the previous step's out; NULL: first-order step
+};
+
+// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; dd = old ? c_cur o - c_old old : o ;
+// x = ratio x - em1 dd ; x = known ? rn n + ry y : x
+__device__ __forceinline__ void multistep_element(float a, float b, float y, float nz, float old, bool known, float& x,
+                                                  float& o, bool combine, float cfg, const lp_multistep& st,
+                                                  bool second, bool next, float rn, float ry) {
+  const float d = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
+  o = known ? y : d;
+  const float dd = second ? __fsub_rn(__fmul_rn(st.c_cur, o), __fmul_rn(st.c_old, old)) : o;
+  x = __fsub_rn(__fmul_rn(st.ratio, x), __fmul_rn(st.em1, dd));
+  if (next) x = known ? fmaf(rn, nz, ry * y) : x;  // rounds as prologue_kernel does
+}
+
+// boundary_kernel's form and operand skipping, x always updated; old is read where x's update survives
+template <int N, typename H, bool kPk>
+__global__ void __launch_bounds__(kBlock) boundary_multistep_kernel(const MultistepArgs q) {
+  pdl_prologue();
+  const BoundaryArgs& p = q.b;
+  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= p.g.total) return;
+  const uint64_t dead = l2_policy_dead(p.l2);
+  uint32_t row, mi;
+  locate(p.g, i, row, mi);
+  const bool next = p.next_table != nullptr, second = q.old != nullptr;
+  float av[N], bv[N], yv[N], xv[N], nv[N], dv[N], ov[N];
+  bool known[N];
+  uint32_t kb = 0, kidx = 0;
+  if constexpr (kPk) {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
+    if constexpr (N == 4) {
+      known_quad(w, i, kb, kidx);
+    } else {
+      kb = (w.x >> (i & 31u)) & 1u;
+      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
+    }
+#pragma unroll
+    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
+  } else {
+    load_m<N>(p.mask, mi, known);
+  }
+  bool any_known = false, any_free = false;
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    any_known |= known[j];
+    any_free |= !known[j];
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = dv[j] = 0.f;
+  if constexpr (kPk) {
+    if constexpr (N == 4) {
+      gather_known4<false>(p.yk, kb, kidx, yv);
+    } else {
+      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
+    }
+  } else {
+    load_f_ro<N>(p.y, i, yv);
+  }
+  if (any_free) {
+    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
+    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
+  }
+  const bool update = any_free || !next;  // somewhere in the vector x's update is not overwritten by the replace step
+  if (update) load_f<N>(p.x, i, xv);
+  if (second && update) load_head_ro<N, float>(q.old, i, dv, dead);  // nothing reads the previous out again
+  float rn = 0.f, ry = 0.f;
+  if (next) {
+    if constexpr (kPk) {
+      if constexpr (N == 4) {
+        gather_known4<false>(p.nk, kb, kidx, nv);
+      } else {
+        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
+      }
+    } else {
+      if (any_known) load_f_ro<N>(p.noise, i, nv);
+    }
+    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
+    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j)
+    multistep_element(av[j], bv[j], yv[j], nv[j], dv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st, second,
+                      next, rn, ry);
+  if (p.out) store_f<N>(p.out, i, ov, dead);
+  store_f<N>(p.x, i, xv);
+  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
+    if (p.discard) {
+      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
+      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
+        __syncwarp();           // every lane's head loads are used
+        discard_line<H>(p.a, i, end);
+        if (p.b) discard_line<H>(p.b, i, end);
+      }
+    }
+  }
+}
+
+template <typename H>
+int multistep_dispatch(const MultistepArgs& q, bool v4, cudaStream_t s) {
+  const uint32_t total = q.b.g.total;
+  if (q.b.kwords) {
+    if (v4) launch_kernel(boundary_multistep_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_multistep_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
+  } else {
+    if (v4) launch_kernel(boundary_multistep_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_multistep_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
+  }
+  return check_launch();
+}
+
+static bool overlaps(const void* p, const void* q, size_t bytes) {
+  const uintptr_t u = reinterpret_cast<uintptr_t>(p), v = reinterpret_cast<uintptr_t>(q);
+  return u < v + bytes && v < u + bytes;
+}
+
+static int boundary_multistep_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                                   const lp_known* known, float* x_inout, float* out, const float* old_out,
+                                   const lp_multistep* step, const float* next_table, const lp_dims* dims,
+                                   lp_stream_t stream) {
+  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
+  if (!x_inout || !step) return LP_ERR_INVALID;
+  MultistepArgs q;
+  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  // the launch writes x and out while it reads old_out
+  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
+  if (old_out && (old_out == x_inout || old_out == out || overlaps(old_out, x_inout, bytes) ||
+                  (out && overlaps(old_out, out, bytes))))
+    return LP_ERR_INVALID;
+  if (q.b.g.total == 0) return LP_OK;
+  boundary_args(q.b, mo, y, noise, mask, known, x_inout, out, 0.f, next_table);
+  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x_inout, out, old_out});  // a dropped line must hold no old_out
+  q.st = *step;
+  q.old = old_out;
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
+  const bool v4 = boundary_vec4(q.b, dtype) && (!old_out || aligned16(old_out));
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (dtype) {
+    case LP_DTYPE_F32: return multistep_dispatch<float>(q, v4, s);
+    case LP_DTYPE_BF16: return multistep_dispatch<__nv_bfloat16>(q, v4, s);
+    default: return multistep_dispatch<__half>(q, v4, s);
+  }
+}
+
 // ---- un-fused OU advance (advance_time_overdamped, lanpaint.py:232-254) --------
 struct AdvanceArgs {
   float* x;
@@ -964,6 +1117,14 @@ extern "C" int lp_boundary_ancestral(const lp_heads* model_out, const float* y, 
                                      const lp_rng* rng, const float* next_table, const lp_dims* dims,
                                      lp_stream_t stream) {
   return boundary_ancestral_impl(model_out, y, noise, mask, known, x_inout, out, step, rng, next_table, dims, stream);
+}
+
+extern "C" int lp_boundary_multistep(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                                     const lp_known* known, float* x_inout, float* out, const float* old_out,
+                                     const lp_multistep* step, const float* next_table, const lp_dims* dims,
+                                     lp_stream_t stream) {
+  return boundary_multistep_impl(model_out, y, noise, mask, known, x_inout, out, old_out, step, next_table, dims,
+                                 stream);
 }
 
 extern "C" int lp_epilogue_f32(const float* model_out, const float* y, const uint8_t* mask, float* out,

@@ -20,7 +20,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _native
-from .schedule import ancestral_step, effective_inner_steps, times_from_sigma
+from .schedule import ancestral_step, dpmpp_2m_step, effective_inner_steps, times_from_sigma
 
 
 class VESampling:
@@ -196,6 +196,21 @@ def euler_ancestral_inpaint(engine, latent_image: torch.Tensor, noise: torch.Ten
     return x
 
 
+def dpmpp_2m_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask, sched: HostSchedule) -> torch.Tensor:
+    """`euler_inpaint` with k-diffusion's sample_dpmpp_2m as the sampler: the un-fused definition of
+    GraphedJob(sampler="dpmpp_2m"), eager torch ops around every wrapper call with the sampler's own scalars
+    (`dpmpp_2m_step` on the schedule, on the latent's device)."""
+    sampling = engine.inner_model.inner_model.model_sampling
+    x = sampling.noise_scaling(sched.sigmas[0].to(latent_image.device), noise, latent_image)
+    old = None
+    for st, (ratio, em1, c_cur, c_old, second) in zip(sched.steps, dpmpp_2m_step(sched.sigmas.to(latent_image.device))):
+        denoised = engine(x, latent_image, noise, st.sigma_t, mask, st.times, None, 0, n_steps=st.n_inner)
+        d = c_cur * denoised - c_old * old if second else denoised
+        x = ratio * x - em1 * d
+        old = denoised
+    return x
+
+
 def time_steady_substep(engine, latent_image: torch.Tensor, mask, sigma: float, launches: int = 53,
                         repeats: int = 20, flow: bool = False, rotate: int = 3):
     """Roofline probe: `launches` steady fused sub-step launches (flags = FUSE_NEXT, the kernel that
@@ -281,15 +296,16 @@ class GraphedJob:
     (src/LanPaint/nodes.py:459 "Recommended: euler").
 
     Semantics are exactly `euler_inpaint(engine, ...)`, i.e. k-diffusion's sample_euler around the
-    per-sigma wrapper (asserted bit-for-bit by the tests)."""
+    per-sigma wrapper (asserted bit-for-bit by the tests); sampler="euler_ancestral" and sampler="dpmpp_2m" are
+    `euler_ancestral_inpaint` and `dpmpp_2m_inpaint`."""
 
     def __init__(self, engine, sched: HostSchedule, shape, device, flow: bool = False, fused_euler: bool = True,
                  l2_persist: bool = False, model_options=None, seed=0, external_init: bool = False,
                  first_replace_noop=None, sampler: str = "euler", eta: float = 1.0, s_noise: float = 1.0):
         import numpy as np
         from .engine import _DrawPlan
-        if sampler not in ("euler", "euler_ancestral"):
-            raise ValueError(f"GraphedJob owns the loops of 'euler' and 'euler_ancestral', not {sampler!r}")
+        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m"):
+            raise ValueError(f"GraphedJob owns the loops of 'euler', 'euler_ancestral' and 'dpmpp_2m', not {sampler!r}")
         self.sampler = sampler
         self.fused_euler = fused_euler   # the sampler's update inside the step-boundary kernel instead of torch kernels
         # optional persisting-L2 window over the clean latent (re-read by every launch).  Off by default: the
@@ -308,6 +324,8 @@ class GraphedJob:
         dev = self.device
         mk = lambda: torch.empty(self.shape, dtype=torch.float32, device=dev)
         self.x, self.y, self.noise, self.c, self.out = mk(), mk(), mk(), mk(), mk()
+        # dpmpp_2m writes every step's denoised latent and reads it back at the next step: two buffers taken in turn
+        self.out_pair = (self.out, mk()) if sampler == "dpmpp_2m" else None
         self.mask = None
         hyper = Hyper(engine.step_size, engine.chara_lamb, engine.chara_beta, engine.min_step_frac, flow)
         tabs, tms, sgs, self.active = [], [], [], []
@@ -333,6 +351,12 @@ class GraphedJob:
                 s_down, s_up = ancestral_step(st.sigma, st.sigma_next, eta)
                 self.ancestral.append((_native.Ancestral(st.sigma, s_down - st.sigma, s_noise, s_up),
                                        st.sigma_next > 0))
+        # dpmpp_2m: one lp_multistep per outer step (the sampler's scalars from its own expressions on this device),
+        # and whether the step is second order, i.e. reads the previous step's denoised latent.  No draw of its own
+        self.multistep = None
+        if sampler == "dpmpp_2m":
+            self.multistep = [(_native.Multistep(ratio, em1, c_cur, c_old), second)
+                              for ratio, em1, c_cur, c_old, second in dpmpp_2m_step(sched.sigmas.to(dev))]
         self.draws_before = [0]
         for i, n in enumerate(self.active):
             own = 1 if (self.ancestral is not None and self.ancestral[i][1]) else 0
@@ -368,6 +392,12 @@ class GraphedJob:
     def per_step_bytes(self) -> int:
         return len(self.sched.steps) * self.x.numel() * 4
 
+    def denoised_buffer(self, i: int, want_out) -> torch.Tensor:
+        """Where outer step i writes its denoised latent (mode "job" with a callback: its own buffer)."""
+        if want_out == "each":
+            return self.outs[i]
+        return self.out_pair[i % 2] if self.out_pair is not None else self.out
+
     # ---- the body ------------------------------------------------------------------------------
     def _init_state(self):
         sampling = self.engine.inner_model.inner_model.model_sampling
@@ -378,23 +408,33 @@ class GraphedJob:
         st = self.sched.steps[i]
         coef = (st.sigma_next - st.sigma) / st.sigma
         anc = self.ancestral[i] if self.ancestral is not None else None
+        ms, old = None, None
+        if self.multistep is not None:
+            ms = self.multistep[i]
+            old = self.denoised_buffer(i - 1, want_out) if ms[1] else None
         last = i + 1 == len(self.sched.steps)
         plan.used = self.draws_before[i]
         out = self.out if (want_out or not self.fused_euler) else None
-        if want_out == "each":      # every outer step keeps its own denoised latent
-            out = self.outs[i]
+        if want_out == "each" or ms is not None:      # every outer step keeps its own denoised latent
+            out = self.denoised_buffer(i, want_out)
         from .engine import heads_discardable
         # the job owns every network call it makes, and the next one overwrites what the last update read
         eng._launch_sequence(self.x, self.y, self.noise, self.mask, self._dims, self.tables[i], self.t_model[i],
                              self.sigma[i], self.c, out, self.active[i], plan, False, self.model_options, self.seed,
                              None, self.rng_state.data_ptr(), discard_heads=heads_discardable(self.model_options),
-                             euler_coef=coef if (self.fused_euler and anc is None) else None,
+                             euler_coef=coef if (self.fused_euler and anc is None and ms is None) else None,
                              skip_prologue=(self.fused_euler and i > 0) or (i == 0 and self.first_replace_noop),
                              next_table=self.tables[i + 1] if (self.fused_euler and not last) else None,
-                             ancestral=anc if self.fused_euler else None)
+                             ancestral=anc if self.fused_euler else None,
+                             multistep=(ms[0], old) if (self.fused_euler and ms is not None) else None)
         if self.fused_euler:
             return
         # un-fused: from this step's denoised latent, wherever it was written
+        if ms is not None:     # sample_dpmpp_2m's tensor ops, in its order
+            step = ms[0]
+            d = out * step.c_cur - old * step.c_old if old is not None else out
+            self.x.mul_(step.ratio).sub_(d * step.em1)
+            return
         if anc is None:
             self.x.add_(self.x - out, alpha=coef)
             return
@@ -531,7 +571,7 @@ class GraphedJob:
                     eng.launches += stats[0]
                     eng.model_calls += stats[1]
                     if callback is not None:
-                        callback(i, self.out, self.x, n_steps)
+                        callback(i, self.denoised_buffer(i, want_out), self.x, n_steps)
             elif mode == "eager":
                 rel = self._relative_plan()
                 if not self.external_init:
@@ -539,7 +579,7 @@ class GraphedJob:
                 for i in range(n_steps):
                     self._step(i, rel, want_out)
                     if callback is not None:
-                        callback(i, self.out, self.x, n_steps)
+                        callback(i, self.denoised_buffer(i, want_out), self.x, n_steps)
             else:
                 raise ValueError(f"unknown mode {mode!r}")
             if self.timing:
@@ -557,9 +597,9 @@ class GraphedJob:
 class SamplerGraphJob:
     """ANY deterministic k-diffusion sampler around the per-sigma wrapper as ONE CUDA graph per job.
 
-    `runner.GraphedJob` owns the sampler loop, so it only serves Euler.  For the other samplers (heun, dpm_2,
-    dpmpp_2m, deis, res_multistep, ...) the loop is third-party Python that calls the wrapper with sigma values only
-    it knows.  But for a fixed schedule that sequence is deterministic: the node layer records it during the first,
+    `runner.GraphedJob` owns the sampler loop, so it only serves the samplers it restates (euler, euler_ancestral,
+    dpmpp_2m).  For the other samplers (heun, dpm_2, deis, res_multistep, ...) the loop is third-party Python that
+    calls the wrapper with sigma values only it knows.  But for a fixed schedule that sequence is deterministic: the node layer records it during the first,
     eager job of a configuration (`KSamplerX0Inpaint.trace`), this class turns every recorded call into device
     constants (`engine.plan_item`) and then runs the sampler function ITSELF under stream capture -- its Python runs
     once, at capture -- with the wrapper serving the planned calls (`engine.run_planned`: no read-back, no copies).

@@ -69,6 +69,35 @@ def ancestral_step(sigma_from: float, sigma_to: float, eta: float = 1.0):
     return s_down, s_up
 
 
+def dpmpp_2m_step(sigmas: torch.Tensor):
+    """[(ratio, em1, c_cur, c_old, second_order)] for every outer step of k-diffusion's sample_dpmpp_2m on `sigmas`.
+
+    The sampler's own torch expressions on its own 0-d fp32 tensors, evaluated where `sigmas` lives (the node hands
+    the sampler a device schedule, so its scalars come from the device's logf / expf / expm1f), then read back once:
+    ratio = sigma_fn(t_next) / sigma_fn(t), em1 = expm1(-h), c_cur = 1 + 1/(2r), c_old = 1/(2r), with t = -log(sigma),
+    h = t_next - t, r = h_last / h.  A step is second order when the sampler has a previous denoised latent and
+    sigma_next != 0; a first-order step has c_cur = c_old = 0 (unused).  The step to sigma = 0 comes out as the sampler
+    computes it: t_next = inf, ratio = 0, em1 = -1."""
+    sigma_fn = lambda t: t.neg().exp()     # noqa: E731
+    t_fn = lambda sigma: sigma.log().neg()  # noqa: E731
+    host = [float(v) for v in sigmas.detach().cpu()]
+    rows = []
+    for i in range(len(host) - 1):
+        t, t_next = t_fn(sigmas[i]), t_fn(sigmas[i + 1])
+        h = t_next - t
+        ratio, em1 = sigma_fn(t_next) / sigma_fn(t), (-h).expm1()
+        second = i > 0 and host[i + 1] != 0.0
+        if second:
+            h_last = t - t_fn(sigmas[i - 1])
+            r = h_last / h
+            c_cur, c_old = 1 + 1 / (2 * r), 1 / (2 * r)
+        else:
+            c_cur = c_old = torch.zeros_like(ratio)
+        rows.append(torch.stack([ratio, em1, c_cur, c_old]))
+    vals = torch.stack(rows).cpu().tolist() if rows else []
+    return [(v[0], v[1], v[2], v[3], i > 0 and host[i + 1] != 0.0) for i, v in enumerate(vals)]
+
+
 @dataclass
 class Hyper:
     step_size: float

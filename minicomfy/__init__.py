@@ -270,7 +270,34 @@ def sample_euler_ancestral(model, x, sigmas, extra_args=None, callback=None, dis
     return x
 
 
-_SAMPLER_FUNCTIONS = {"euler": sample_euler, "heun": sample_heun, "euler_ancestral": sample_euler_ancestral}
+@torch.no_grad()
+def sample_dpmpp_2m(model, x, sigmas, extra_args=None, callback=None, disable=None):
+    """k-diffusion's DPM-Solver++(2M): a second-order multistep update from this step's and the previous step's
+    denoised latents, first order on the first step and on the step to sigma = 0."""
+    extra_args = extra_args or {}
+    s_in = x.new_ones([x.shape[0]])
+    sigma_fn = lambda t: t.neg().exp()     # noqa: E731
+    t_fn = lambda sigma: sigma.log().neg()  # noqa: E731
+    old_denoised = None
+    for i in range(len(sigmas) - 1):
+        denoised = model(x, sigmas[i] * s_in, **extra_args)
+        if callback is not None:
+            callback({"x": x, "i": i, "sigma": sigmas[i], "sigma_hat": sigmas[i], "denoised": denoised})
+        t, t_next = t_fn(sigmas[i]), t_fn(sigmas[i + 1])
+        h = t_next - t
+        if old_denoised is None or sigmas[i + 1] == 0:
+            x = (sigma_fn(t_next) / sigma_fn(t)) * x - (-h).expm1() * denoised
+        else:
+            h_last = t - t_fn(sigmas[i - 1])
+            r = h_last / h
+            denoised_d = (1 + 1 / (2 * r)) * denoised - (1 / (2 * r)) * old_denoised
+            x = (sigma_fn(t_next) / sigma_fn(t)) * x - (-h).expm1() * denoised_d
+        old_denoised = denoised
+    return x
+
+
+_SAMPLER_FUNCTIONS = {"euler": sample_euler, "heun": sample_heun, "euler_ancestral": sample_euler_ancestral,
+                      "dpmpp_2m": sample_dpmpp_2m}
 
 
 class KSAMPLER:
