@@ -33,7 +33,9 @@ extern "C" {
 #define LP_ABI_VERSION 5
 /* Backward-compatible additions within LP_ABI_VERSION: 1 = LP_HEADS_DEAD (a dtype bit every earlier library
  * rejected with LP_ERR_INVALID, so no earlier caller can have set it); 2 = lp_multistep and
- * lp_boundary_multistep (a new entry point: nothing an earlier caller binds changes). */
+ * lp_boundary_multistep (a new entry point: nothing an earlier caller binds changes).  Later entry points
+ * (lp_midpoint and lp_boundary_midpoint) leave LP_ABI_MINOR at 2: a caller detects one by its symbol, which is
+ * how lanpaint_b200._native binds every entry point (by name). */
 #define LP_ABI_MINOR 2
 #define LP_TABLE_STRIDE 32 /* floats per table row (one 128-byte line), layout below */
 
@@ -396,6 +398,33 @@ typedef struct lp_multistep {
 int lp_boundary_multistep(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                           const lp_known* known, float* x_inout, float* out, const float* old_out,
                           const lp_multistep* step, const float* next_table, const lp_dims* dims, lp_stream_t stream);
+
+/* One update of k-diffusion's sample_dpm_2 (DPM-Solver-2, no churn): x_out = x_base + ((x_in - out) / sigma) * dt.
+ * The host evaluates sigma and dt with the sampler's own torch expressions on the schedule, on the device the
+ * sampler runs on, and reads them back.  Per outer step i with sigma_next > 0:
+ *   predictor  sigma = sigma_i,   dt = sigma_mid - sigma_i    x_in = x_base = X,  x_out = X2
+ *   corrector  sigma = sigma_mid, dt = sigma_next - sigma_i   x_in = X2, x_base = x_out = X
+ * with sigma_mid = exp(lerp(log sigma_i, log sigma_next, 1/2)); the step to sigma_next = 0 is one Euler update,
+ * sigma = sigma_i, dt = -sigma_i, x_in = x_base = x_out = X. */
+typedef struct lp_midpoint {
+  float sigma; /* the sigma the update divides by */
+  float dt;    /* the step it multiplies with */
+} lp_midpoint;
+
+/* The boundary of a wrapper call of a host-owned DPM-Solver-2 loop in ONE pass: lp_boundary_known with the Euler
+ * update replaced by sample_dpm_2's:
+ *   d     = model_out->combine ? b + (a - b)*cfg : a
+ *   out   = mask ? y : d                                                written when out != NULL
+ *   x_out = x_base + ((x_in - out) / sigma) * dt
+ *   x_out = mask ? rep_noise*noise + rep_y*y : x_out  (row of next_table)  when next_table != NULL
+ * Every operation of the update is the single correctly rounded fp32 operation the eager sampler issues (sub, div,
+ * mul, add; never contracted), so x_out equals the un-fused route's bit for bit.  x_in and x_base are read only where
+ * the update survives (free positions; known positions too when next_table == NULL), once when they are the same
+ * pointer.  Any two of x_in, x_base and x_out are the same buffer or disjoint; out overlaps none of them.  known may
+ * be NULL (dense y / noise / mask). */
+int lp_boundary_midpoint(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                         const lp_known* known, const float* x_in, const float* x_base, float* x_out, float* out,
+                         const lp_midpoint* step, const float* next_table, const lp_dims* dims, lp_stream_t stream);
 
 /* Final denoise of an outer step straight from raw cond / uncond predictions:
  *   out = mask ? y : uncond + (cond - uncond)*cfg ;  if x_inout != NULL: x = x + (x - out)*euler_coef. */

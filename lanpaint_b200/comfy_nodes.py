@@ -391,7 +391,8 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         with ComfyUI's callback between them when the job is long enough to watch) cached across sample() calls;
         with the option "fused_ancestral" the same holds for euler_ancestral, whose step and randn_like draw
         run inside lp_boundary_ancestral; dpmpp_2m runs there too (on by default), its update and the previous
-        step's denoised latent inside lp_boundary_multistep;
+        step's denoised latent inside lp_boundary_multistep, and so does dpm_2 (on by default), both of its wrapper
+        calls per step in the loop and both of its updates inside lp_boundary_midpoint;
       * any other deterministic sampler: the first job records which sigmas the sampler hands the wrapper, then
         k-diffusion's sampler function itself is captured into ONE graph (`runner.SamplerGraphJob`);
       * anything else (samplers that draw their own noise, early stop, AV packs, mask schedules): k-diffusion's own
@@ -464,17 +465,20 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             timing[0].record()
 
         samples = None
-        ancestral = None
+        fused = None      # the runner.GraphedJob sampler kwargs of the host-owned loop this sampler maps onto
         if opts.get("fused_ancestral", False) and KSAMPLER._fused_ancestral_ok(self, model_k, denoise_mask, model_options,
                                                                                 engine):
-            ancestral = sampler_key[1:]
-        multistep = ancestral is None and KSAMPLER._fused_dpmpp_2m_ok(self, model_k, denoise_mask, model_options,
-                                                                      engine)
-        if opts.get("fused_sampler", True) and (ancestral is not None or multistep or KSAMPLER._fused_euler_ok(
-                self, model_k, denoise_mask, model_options, engine)):
+            fused = dict(sampler="euler_ancestral", eta=sampler_key[1], s_noise=sampler_key[2])
+        elif KSAMPLER._fused_dpmpp_2m_ok(self, model_k, denoise_mask, model_options, engine):
+            fused = dict(sampler="dpmpp_2m")
+        elif KSAMPLER._fused_dpm_2_ok(self, model_k, denoise_mask, model_options, engine):
+            fused = dict(sampler="dpm_2")
+        elif KSAMPLER._fused_euler_ok(self, model_k, denoise_mask, model_options, engine):
+            fused = {}
+        if opts.get("fused_sampler", True) and fused is not None:
             samples = KSAMPLER._fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options,
                                         extra_args.get("seed"), is_flux or is_flow, early_stop, callback, total_steps,
-                                        use_graph, opts, ancestral, multistep)
+                                        use_graph, opts, fused)
         sg_ok = False
         if samples is None and use_graph and entry is not None and opts.get("sampler_graph", True):
             sg_ok = KSAMPLER._sampler_graph_ok(self, model_k, denoise_mask, model_options, engine, entry)
@@ -562,8 +566,17 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             return False
         return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
 
+    def _fused_dpm_2_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
+        """True when k-diffusion's sample_dpm_2 around the per-sigma wrapper is the host-owned loop of
+        runner.GraphedJob(sampler="dpm_2"): the sampler without extra options (no churn), and the exclusions of
+        `_fused_euler_ok`."""
+        if getattr(self.sampler_function, "__name__", "") != "sample_dpm_2" or self.extra_options:
+            return False
+        return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
+
     def _fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options, seed, flow,
-                     early_stop, callback, total_steps, use_graph, opts, ancestral=None, multistep=False):
+                     early_stop, callback, total_steps, use_graph, opts, sampler=None):
+        """sampler: the GraphedJob sampler kwargs (None or {}: plain Euler)."""
         from .runner import GraphedJob, HostSchedule
         if not x_init.is_cuda:
             raise RuntimeError("lanpaint_b200 needs the latent on a CUDA device: there is no CPU or eager fallback")
@@ -574,12 +587,8 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         if job is None:
             sched = HostSchedule(model_k.sigmas_host, B, engine.n_steps, flow, early_stop, engine.min_step_frac)
             try:
-                sampler = {} if ancestral is None else dict(sampler="euler_ancestral", eta=ancestral[0],
-                                                            s_noise=ancestral[1])
-                if multistep:
-                    sampler = dict(sampler="dpmpp_2m")
                 job = GraphedJob(engine, sched, tuple(x_init.shape), x_init.device, flow=flow, external_init=True,
-                                 first_replace_noop=False, **sampler)
+                                 first_replace_noop=False, **(sampler or {}))
             except ValueError:     # noise_scaling is not a linear form: the per-sigma wrapper calls it instead
                 return None
             if entry is not None:

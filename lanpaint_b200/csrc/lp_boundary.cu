@@ -6,6 +6,8 @@
 //                       the same boundary for k-diffusion's sample_euler_ancestral, its randn_like drawn in-kernel
 //   boundary_multistep_kernel
 //                       the same boundary for k-diffusion's sample_dpmpp_2m (DPM-Solver++(2M))
+//   boundary_midpoint_kernel
+//                       the same boundary for either wrapper call of k-diffusion's sample_dpm_2 (DPM-Solver-2)
 //   advance_kernel      one un-fused advance_time_overdamped             lanpaint.py:232-254
 //   stop_stats_kernel   early-stop masked reductions                     earlystop.py:32-55,238-313
 #include "lp_common.cuh"
@@ -946,6 +948,164 @@ static int boundary_multistep_impl(const lp_heads* mo, const float* y, const flo
   }
 }
 
+// ---- the boundary of a wrapper call of a host-owned DPM-Solver-2 loop ------------------------------------------
+// k-diffusion's sample_dpm_2 issues, after each wrapper call, sub, div, mul, add as eager kernels, with per-step 0-d
+// tensors the host hands in as lp_midpoint; lp_boundary_midpoint does them in the boundary's one pass, each as the
+// same correctly rounded fp32 operation.
+struct MidpointArgs {
+  BoundaryArgs b;       // b.x is x_out; coef is unused
+  lp_midpoint st;
+  const float* xin;
+  const float* xbase;   // == xin: read once
+  int evict;            // x_in / x_base are not read again before a whole network call: load them evict-first
+};
+
+// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; x = base + ((in - o) / sigma) dt ;
+// x = known ? rn n + ry y : x
+__device__ __forceinline__ void midpoint_element(float a, float b, float y, float nz, float in, float base, bool known,
+                                                 float& x, float& o, bool combine, float cfg, const lp_midpoint& st,
+                                                 bool next, float rn, float ry) {
+  const float d = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
+  o = known ? y : d;
+  x = __fadd_rn(base, __fmul_rn(__fdiv_rn(__fsub_rn(in, o), st.sigma), st.dt));
+  if (next) x = known ? fmaf(rn, nz, ry * y) : x;  // rounds as prologue_kernel does
+}
+
+// boundary_kernel's form and operand skipping; x_in and x_base are read where x_out's update survives
+template <int N, typename H, bool kPk>
+__global__ void __launch_bounds__(kBlock) boundary_midpoint_kernel(const MidpointArgs q) {
+  pdl_prologue();
+  const BoundaryArgs& p = q.b;
+  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= p.g.total) return;
+  const uint64_t dead = l2_policy_dead(p.l2);
+  uint32_t row, mi;
+  locate(p.g, i, row, mi);
+  const bool next = p.next_table != nullptr;
+  float av[N], bv[N], yv[N], nv[N], iv[N], sv[N], xv[N], ov[N];
+  bool known[N];
+  uint32_t kb = 0, kidx = 0;
+  if constexpr (kPk) {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
+    if constexpr (N == 4) {
+      known_quad(w, i, kb, kidx);
+    } else {
+      kb = (w.x >> (i & 31u)) & 1u;
+      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
+    }
+#pragma unroll
+    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
+  } else {
+    load_m<N>(p.mask, mi, known);
+  }
+  bool any_known = false, any_free = false;
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    any_known |= known[j];
+    any_free |= !known[j];
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) av[j] = bv[j] = nv[j] = iv[j] = sv[j] = 0.f;
+  if constexpr (kPk) {
+    if constexpr (N == 4) {
+      gather_known4<false>(p.yk, kb, kidx, yv);
+    } else {
+      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
+    }
+  } else {
+    load_f_ro<N>(p.y, i, yv);
+  }
+  if (any_free) {
+    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
+    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
+  }
+  if (any_free || !next) {  // somewhere in the vector x_out's update is not overwritten by the replace step
+    const uint64_t xp = q.evict ? dead : 0;
+    load_f<N>(q.xin, i, iv, xp);
+    if (q.xbase != q.xin) {
+      load_f<N>(q.xbase, i, sv, xp);
+    } else {
+#pragma unroll
+      for (int j = 0; j < N; ++j) sv[j] = iv[j];
+    }
+  }
+  float rn = 0.f, ry = 0.f;
+  if (next) {
+    if constexpr (kPk) {
+      if constexpr (N == 4) {
+        gather_known4<false>(p.nk, kb, kidx, nv);
+      } else {
+        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
+      }
+    } else {
+      if (any_known) load_f_ro<N>(p.noise, i, nv);
+    }
+    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
+    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j)
+    midpoint_element(av[j], bv[j], yv[j], nv[j], iv[j], sv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st,
+                     next, rn, ry);
+  if (p.out) store_f<N>(p.out, i, ov, dead);
+  store_f<N>(p.x, i, xv);  // normal policy: the next network call reads x_out first
+  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
+    if (p.discard) {
+      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
+      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
+        __syncwarp();           // every lane's head loads are used
+        discard_line<H>(p.a, i, end);
+        if (p.b) discard_line<H>(p.b, i, end);
+      }
+    }
+  }
+}
+
+template <typename H>
+int midpoint_dispatch(const MidpointArgs& q, bool v4, cudaStream_t s) {
+  const uint32_t total = q.b.g.total;
+  if (q.b.kwords) {
+    if (v4) launch_kernel(boundary_midpoint_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_midpoint_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
+  } else {
+    if (v4) launch_kernel(boundary_midpoint_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_midpoint_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
+  }
+  return check_launch();
+}
+
+static int boundary_midpoint_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                                  const lp_known* known, const float* x_in, const float* x_base, float* x_out,
+                                  float* out, const lp_midpoint* step, const float* next_table, const lp_dims* dims,
+                                  lp_stream_t stream) {
+  if (int rc = boundary_check(mo, y, noise, mask, known, x_out, out, next_table)) return rc;
+  if (!step || !x_in || !x_base || !x_out) return LP_ERR_INVALID;
+  MidpointArgs q;
+  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  // one thread reads and writes each element: the three states are each one buffer or disjoint, and out, which the
+  // launch writes, shares no byte with any of them
+  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
+  const auto partial = [&](const void* u, const void* v) { return u != v && overlaps(u, v, bytes); };
+  const auto any = [&](const void* u, const void* v) { return u == v || overlaps(u, v, bytes); };
+  if (partial(x_in, x_base) || partial(x_in, x_out) || partial(x_base, x_out)) return LP_ERR_INVALID;
+  if (out && (any(out, x_in) || any(out, x_base) || any(out, x_out))) return LP_ERR_INVALID;
+  if (q.b.g.total == 0) return LP_OK;
+  boundary_args(q.b, mo, y, noise, mask, known, x_out, out, 0.f, next_table);
+  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x_in, x_base, x_out, out});  // a dropped line holds no state
+  q.st = *step;
+  q.xin = x_in;
+  q.xbase = x_base;
+  q.evict = !(x_in == x_out && x_base == x_out);  // the predictor's X, the corrector's X2 and X
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
+  const bool v4 = boundary_vec4(q.b, dtype) && aligned16(x_in) && aligned16(x_base);
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (dtype) {
+    case LP_DTYPE_F32: return midpoint_dispatch<float>(q, v4, s);
+    case LP_DTYPE_BF16: return midpoint_dispatch<__nv_bfloat16>(q, v4, s);
+    default: return midpoint_dispatch<__half>(q, v4, s);
+  }
+}
+
 // ---- un-fused OU advance (advance_time_overdamped, lanpaint.py:232-254) --------
 struct AdvanceArgs {
   float* x;
@@ -1125,6 +1285,14 @@ extern "C" int lp_boundary_multistep(const lp_heads* model_out, const float* y, 
                                      lp_stream_t stream) {
   return boundary_multistep_impl(model_out, y, noise, mask, known, x_inout, out, old_out, step, next_table, dims,
                                  stream);
+}
+
+extern "C" int lp_boundary_midpoint(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                                    const lp_known* known, const float* x_in, const float* x_base, float* x_out,
+                                    float* out, const lp_midpoint* step, const float* next_table, const lp_dims* dims,
+                                    lp_stream_t stream) {
+  return boundary_midpoint_impl(model_out, y, noise, mask, known, x_in, x_base, x_out, out, step, next_table, dims,
+                                stream);
 }
 
 extern "C" int lp_epilogue_f32(const float* model_out, const float* y, const uint8_t* mask, float* out,

@@ -20,7 +20,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _native
-from .schedule import ancestral_step, dpmpp_2m_step, effective_inner_steps, times_from_sigma
+from .schedule import ancestral_step, dpm_2_step, dpmpp_2m_step, effective_inner_steps, times_from_sigma
 
 
 class VESampling:
@@ -127,6 +127,7 @@ class HostSchedule:
         sig = torch.as_tensor(list(sigmas), dtype=torch.float32)
         self.sigmas = sig
         host = [float(v) for v in sig]
+        self._call = (batch, n_inner, flow, early_stop, min_step_frac)
         self.steps: List[OuterStep] = []
         ones = torch.ones(batch, dtype=torch.float32)
         for i in range(len(host) - 1):
@@ -137,6 +138,16 @@ class HostSchedule:
             self.steps.append(OuterStep(host[i], host[i + 1], n_eff, s, tm))
         self.substeps = sum(st.n_inner for st in self.steps)
         self.model_calls = self.substeps + len(self.steps)
+
+    def call_at(self, sigma: float, sigma_next: float) -> OuterStep:
+        """The row of a wrapper call at a sigma that need not be in the schedule (sample_dpm_2's midpoint): what the
+        per-sigma wrapper derives from it -- sigma * ones[B], the times, and n_eff by its nearest-sigma rule."""
+        batch, n_inner, flow, early_stop, min_step_frac = self._call
+        s = torch.tensor(sigma, dtype=torch.float32) * torch.ones(batch, dtype=torch.float32)
+        tm = times_from_sigma(s, flow)
+        n_eff = effective_inner_steps(n_inner, [float(v) for v in self.sigmas], float(torch.mean(s)),
+                                      float((1.0 - tm[1]).mean()), early_stop, min_step_frac)
+        return OuterStep(float(s[0]), sigma_next, n_eff, s, tm)
 
 
 def karras_sigmas(n: int, sigma_min: float = 0.0292, sigma_max: float = 14.6146, rho: float = 7.0) -> List[float]:
@@ -208,6 +219,28 @@ def dpmpp_2m_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, ma
         d = c_cur * denoised - c_old * old if second else denoised
         x = ratio * x - em1 * d
         old = denoised
+    return x
+
+
+def dpm_2_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask, sched: HostSchedule) -> torch.Tensor:
+    """`euler_inpaint` with k-diffusion's sample_dpm_2 (no churn) as the sampler: the un-fused definition of
+    GraphedJob(sampler="dpm_2"), eager torch ops around both wrapper calls of a step with the sampler's own scalars
+    (`dpm_2_step` on the schedule, on the latent's device); the midpoint call's row is `HostSchedule.call_at`."""
+    dev = latent_image.device
+    sampling = engine.inner_model.inner_model.model_sampling
+    sig = sched.sigmas.to(dev)
+    x = sampling.noise_scaling(sig[0], noise, latent_image)
+    for i, (st, (s_mid, dt_1, dt_2, mid)) in enumerate(zip(sched.steps, dpm_2_step(sig))):
+        sigma_hat = sig[i] * (0.0 + 1)
+        denoised = engine(x, latent_image, noise, st.sigma_t, mask, st.times, None, 0, n_steps=st.n_inner)
+        d = (x - denoised) / sigma_hat
+        if not mid:
+            x = x + d * torch.tensor(dt_2, device=dev)
+            continue
+        x_2 = x + d * torch.tensor(dt_1, device=dev)
+        ms = sched.call_at(s_mid, st.sigma_next)
+        denoised_2 = engine(x_2, latent_image, noise, ms.sigma_t, mask, ms.times, None, 0, n_steps=ms.n_inner)
+        x = x + ((x_2 - denoised_2) / torch.tensor(s_mid, device=dev)) * torch.tensor(dt_2, device=dev)
     return x
 
 
@@ -296,16 +329,18 @@ class GraphedJob:
     (src/LanPaint/nodes.py:459 "Recommended: euler").
 
     Semantics are exactly `euler_inpaint(engine, ...)`, i.e. k-diffusion's sample_euler around the
-    per-sigma wrapper (asserted bit-for-bit by the tests); sampler="euler_ancestral" and sampler="dpmpp_2m" are
-    `euler_ancestral_inpaint` and `dpmpp_2m_inpaint`."""
+    per-sigma wrapper (asserted bit-for-bit by the tests); sampler="euler_ancestral", "dpmpp_2m" and "dpm_2" are
+    `euler_ancestral_inpaint`, `dpmpp_2m_inpaint` and `dpm_2_inpaint`.  dpm_2 makes two wrapper calls per outer step:
+    call A at sigma_i on x, call B at the midpoint sigma on a second state buffer x2; both are in the step's graph."""
 
     def __init__(self, engine, sched: HostSchedule, shape, device, flow: bool = False, fused_euler: bool = True,
                  l2_persist: bool = False, model_options=None, seed=0, external_init: bool = False,
                  first_replace_noop=None, sampler: str = "euler", eta: float = 1.0, s_noise: float = 1.0):
         import numpy as np
         from .engine import _DrawPlan
-        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m"):
-            raise ValueError(f"GraphedJob owns the loops of 'euler', 'euler_ancestral' and 'dpmpp_2m', not {sampler!r}")
+        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m", "dpm_2"):
+            raise ValueError("GraphedJob owns the loops of 'euler', 'euler_ancestral', 'dpmpp_2m' and 'dpm_2', "
+                             f"not {sampler!r}")
         self.sampler = sampler
         self.fused_euler = fused_euler   # the sampler's update inside the step-boundary kernel instead of torch kernels
         # optional persisting-L2 window over the clean latent (re-read by every launch).  Off by default: the
@@ -326,19 +361,28 @@ class GraphedJob:
         self.x, self.y, self.noise, self.c, self.out = mk(), mk(), mk(), mk(), mk()
         # dpmpp_2m writes every step's denoised latent and reads it back at the next step: two buffers taken in turn
         self.out_pair = (self.out, mk()) if sampler == "dpmpp_2m" else None
+        # dpm_2: the midpoint call's state (x_2 of the sampler)
+        self.x2 = mk() if sampler == "dpm_2" else None
         self.mask = None
         hyper = Hyper(engine.step_size, engine.chara_lamb, engine.chara_beta, engine.min_step_frac, flow)
-        tabs, tms, sgs, self.active = [], [], [], []
-        for st in sched.steps:
+
+        def call_row(st):
+            """(table, model time, sigma, active sub-steps) of one wrapper call"""
             ve, abt, flow_t = (t.numpy() for t in st.times)
             sig = st.sigma_t.numpy()
             form = engine._replace_form(sig, st.sigma_t.numel() == 1, B, engine.replace_mode, engine.batched_replace)
             if form is None:
                 raise ValueError("model_sampling.noise_scaling is not a linear form; GraphedJob cannot precompute it")
-            tabs.append(build_table(abt, ve, hyper, form[0], form[1]))
-            tms.append(flow_t if flow else ve)
+            return (build_table(abt, ve, hyper, form[0], form[1]), flow_t if flow else ve, sig,
+                    st.n_inner if mean_half_dt(abt, hyper) > 0.0 else 0)
+
+        tabs, tms, sgs, self.active = [], [], [], []
+        for st in sched.steps:
+            tab, tm, sig, active = call_row(st)
+            tabs.append(tab)
+            tms.append(tm)
             sgs.append(sig)
-            self.active.append(st.n_inner if mean_half_dt(abt, hyper) > 0.0 else 0)
+            self.active.append(active)
         # draws consumed before outer step i (1 for sub-step 0, 2 for each later one): lets every outer step be
         # captured on its own against ONE {seed, base} block that is refreshed once per job
         merged = engine.rng == "philox" and engine.merge_noise   # a fused launch then draws ONE normal, not two
@@ -357,10 +401,37 @@ class GraphedJob:
         if sampler == "dpmpp_2m":
             self.multistep = [(_native.Multistep(ratio, em1, c_cur, c_old), second)
                               for ratio, em1, c_cur, c_old, second in dpmpp_2m_step(sched.sigmas.to(dev))]
+        # dpm_2: per outer step (lp_midpoint of call A's update, of call B's or None, the index of call B's row), the
+        # rows of the midpoint calls (their own tables, model times, sigmas and active counts), and the sampler's
+        # scalars as device tensors for the un-fused update.  No draw of its own
+        self.midpoint = None
+        self.substeps = sched.substeps
+        if sampler == "dpm_2":
+            self.midpoint, mrows = [], []
+            for i, (st, (s_mid, dt_1, dt_2, mid)) in enumerate(zip(sched.steps, dpm_2_step(sched.sigmas.to(dev)))):
+                if not mid:
+                    self.midpoint.append((_native.Midpoint(st.sigma, dt_2), None, None))
+                    continue
+                ms = sched.call_at(s_mid, st.sigma_next)
+                self.substeps += ms.n_inner
+                self.midpoint.append((_native.Midpoint(st.sigma, dt_1), _native.Midpoint(s_mid, dt_2), len(mrows)))
+                mrows.append(call_row(ms))
+            col = lambda j: (torch.from_numpy(np.stack([r[j] for r in mrows]).astype(np.float32)).to(dev)  # noqa: E731
+                             if mrows else None)
+            self.mid_tables, self.mid_t_model, self.mid_sigma = col(0), col(1), col(2)
+            self.mid_active = [r[3] for r in mrows]
+            self.dpm_2_scalars = torch.tensor([[st.sigma, a.dt, b.sigma if b else 0.0, b.dt if b else 0.0]
+                                               for st, (a, b, _) in zip(sched.steps, self.midpoint)],
+                                              dtype=torch.float32, device=dev)
+            self.out_mid = mk() if not fused_euler else None   # the midpoint call's denoised latent (un-fused update)
+        draws = lambda n: 0 if n <= 0 else (n if merged else 2 * n - 1)   # noqa: E731  one wrapper call's draws
+        self._call_draws = draws
         self.draws_before = [0]
         for i, n in enumerate(self.active):
             own = 1 if (self.ancestral is not None and self.ancestral[i][1]) else 0
-            self.draws_before.append(self.draws_before[-1] + (0 if n <= 0 else (n if merged else 2 * n - 1)) + own)
+            if self.midpoint is not None and self.midpoint[i][2] is not None:
+                own = draws(self.mid_active[self.midpoint[i][2]])     # call B's Langevin draws
+            self.draws_before.append(self.draws_before[-1] + draws(n) + own)
         self.tables = torch.from_numpy(np.stack(tabs)).to(dev)
         self.t_model = torch.from_numpy(np.stack(tms).astype(np.float32)).to(dev)
         self.sigma = torch.from_numpy(np.stack(sgs).astype(np.float32)).to(dev)
@@ -404,6 +475,8 @@ class GraphedJob:
         self.x.copy_(sampling.noise_scaling(self.sigma0, self.noise, self.y))
 
     def _step(self, i, plan, want_out):
+        if self.midpoint is not None:
+            return self._dpm_2_step(i, plan, want_out)
         eng = self.engine
         st = self.sched.steps[i]
         coef = (st.sigma_next - st.sigma) / st.sigma
@@ -448,6 +521,47 @@ class GraphedJob:
                                                    C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
             _native.check(rc, "lp_fill_normal_f32")
             self.x.add_(xi * step.s_noise * step.sigma_up)
+
+    def _dpm_2_step(self, i, plan, want_out):
+        """Outer step i of sample_dpm_2: call A at sigma_i on x, then (sigma_next > 0) call B at sigma_mid on x2.
+        Fused, call A's boundary is the predictor (x -> x2) with call B's replace step (its row) folded in, and call
+        B's boundary is the corrector (x2, x -> x) with the next outer step's replace step; the step to sigma = 0 is
+        one Euler boundary on x."""
+        from .engine import heads_discardable
+        eng = self.engine
+        pred, corr, k = self.midpoint[i]
+        last = i + 1 == len(self.sched.steps)
+        fused = self.fused_euler
+        after = self.tables[i + 1] if not last else None     # the next outer step's replace step
+        plan.used = self.draws_before[i]
+        out = self.out if (want_out or not fused) else None
+        if want_out == "each":
+            out = self.outs[i]
+        dead = heads_discardable(self.model_options)
+        common = (self.y, self.noise, self.mask, self._dims)
+        x_a = self.x2 if k is not None else self.x
+        eng._launch_sequence(self.x, *common, self.tables[i], self.t_model[i], self.sigma[i], self.c, out,
+                             self.active[i], plan, False, self.model_options, self.seed, None,
+                             self.rng_state.data_ptr(), discard_heads=dead,
+                             skip_prologue=(fused and i > 0) or (i == 0 and self.first_replace_noop),
+                             next_table=(self.mid_tables[k] if k is not None else after) if fused else None,
+                             midpoint=(pred, self.x, x_a) if fused else None)
+        sc = self.dpm_2_scalars[i]
+        if not fused:   # sample_dpm_2's tensor ops, in its order
+            d = (self.x - out) / sc[0]
+            if k is None:
+                self.x.add_(d * sc[1])
+                return
+            torch.add(self.x, d * sc[1], out=self.x2)
+        if k is None:
+            return
+        plan.used = self.draws_before[i] + self._call_draws(self.active[i])
+        eng._launch_sequence(self.x2, *common, self.mid_tables[k], self.mid_t_model[k], self.mid_sigma[k], self.c,
+                             None if fused else self.out_mid, self.mid_active[k], plan, False, self.model_options,
+                             self.seed, None, self.rng_state.data_ptr(), discard_heads=dead, skip_prologue=fused,
+                             next_table=after if fused else None, midpoint=(corr, self.x, self.x) if fused else None)
+        if not fused:
+            self.x.add_(((self.x2 - self.out_mid) / sc[2]) * sc[3])
 
     def _body(self, plan, want_out):
         if not self.external_init:
@@ -586,7 +700,7 @@ class GraphedJob:
                 self.last_events[1].record()
             plan.consume(self.draws)
             plan.finish()
-            eng.substeps_done += self.sched.substeps
+            eng.substeps_done += self.substeps
             self.launches, self.model_calls = eng.launches - before[0], eng.model_calls - before[1]
             if x_out is not None:
                 x_out.copy_(self.x, non_blocking=True)
@@ -598,7 +712,7 @@ class SamplerGraphJob:
     """ANY deterministic k-diffusion sampler around the per-sigma wrapper as ONE CUDA graph per job.
 
     `runner.GraphedJob` owns the sampler loop, so it only serves the samplers it restates (euler, euler_ancestral,
-    dpmpp_2m).  For the other samplers (heun, dpm_2, deis, res_multistep, ...) the loop is third-party Python that
+    dpmpp_2m, dpm_2).  For the other samplers (heun, deis, res_multistep, ...) the loop is third-party Python that
     calls the wrapper with sigma values only it knows.  But for a fixed schedule that sequence is deterministic: the node layer records it during the first,
     eager job of a configuration (`KSamplerX0Inpaint.trace`), this class turns every recorded call into device
     constants (`engine.plan_item`) and then runs the sampler function ITSELF under stream capture -- its Python runs

@@ -98,6 +98,27 @@ def dpmpp_2m_step(sigmas: torch.Tensor):
     return [(v[0], v[1], v[2], v[3], i > 0 and host[i + 1] != 0.0) for i, v in enumerate(vals)]
 
 
+def dpm_2_step(sigmas: torch.Tensor):
+    """[(sigma_mid, dt_1, dt_2, midpoint)] for every outer step of k-diffusion's sample_dpm_2 (no churn) on `sigmas`.
+
+    As `dpmpp_2m_step`: the sampler's own torch expressions on its own 0-d fp32 tensors where `sigmas` lives, read back
+    once.  With sigma_hat = sigma_i: sigma_mid = exp(lerp(log sigma_hat, log sigma_next, 1/2)), dt_1 = sigma_mid -
+    sigma_hat, dt_2 = sigma_next - sigma_hat.  A step makes its midpoint call when sigma_next != 0; the step to
+    sigma = 0 is one Euler update with dt_2 = sigma_next - sigma_hat, and sigma_mid = dt_1 = 0 (unused)."""
+    host = [float(v) for v in sigmas.detach().cpu()]
+    rows = []
+    for i in range(len(host) - 1):
+        sigma_hat = sigmas[i] * (0.0 + 1)
+        dt_2 = sigmas[i + 1] - sigma_hat
+        if host[i + 1] != 0.0:
+            sigma_mid = sigma_hat.log().lerp(sigmas[i + 1].log(), 0.5).exp()
+            rows.append(torch.stack([sigma_mid, sigma_mid - sigma_hat, dt_2]))
+        else:
+            rows.append(torch.stack([torch.zeros_like(dt_2), torch.zeros_like(dt_2), dt_2]))
+    vals = torch.stack(rows).cpu().tolist() if rows else []
+    return [(v[0], v[1], v[2], host[i + 1] != 0.0) for i, v in enumerate(vals)]
+
+
 @dataclass
 class Hyper:
     step_size: float

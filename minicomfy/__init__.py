@@ -296,8 +296,36 @@ def sample_dpmpp_2m(model, x, sigmas, extra_args=None, callback=None, disable=No
     return x
 
 
+@torch.no_grad()
+def sample_dpm_2(model, x, sigmas, extra_args=None, callback=None, disable=None):
+    """k-diffusion's DPM-Solver-2 without churn: an Euler step to the log-midpoint of sigma and sigma_next, a second
+    model call there, and the step from sigma to sigma_next with that call's derivative; plain Euler to sigma = 0."""
+    extra_args = extra_args or {}
+    s_in = x.new_ones([x.shape[0]])
+    for i in range(len(sigmas) - 1):
+        sigma_hat = sigmas[i] * (0.0 + 1)
+        denoised = model(x, sigma_hat * s_in, **extra_args)
+        d = (x - denoised) / _append_dims(sigma_hat, x.ndim)
+        if callback is not None:
+            callback({"x": x, "i": i, "sigma": sigmas[i], "sigma_hat": sigma_hat, "denoised": denoised})
+        if sigmas[i + 1] == 0:
+            dt = sigmas[i + 1] - sigma_hat
+            x = x + d * dt
+        else:
+            sigma_mid = sigma_hat.log().lerp(sigmas[i + 1].log(), 0.5).exp()
+            dt_1 = sigma_mid - sigma_hat
+            dt_2 = sigmas[i + 1] - sigma_hat
+            x_2 = x + d * dt_1
+            denoised_2 = model(x_2, sigma_mid * s_in, **extra_args)
+            d_2 = (x_2 - denoised_2) / _append_dims(sigma_mid, x.ndim)
+            x = x + d_2 * dt_2
+    return x
+
+
 _SAMPLER_FUNCTIONS = {"euler": sample_euler, "heun": sample_heun, "euler_ancestral": sample_euler_ancestral,
-                      "dpmpp_2m": sample_dpmpp_2m}
+                      "dpmpp_2m": sample_dpmpp_2m, "dpm_2": sample_dpm_2}
+# ComfyUI's KSampler takes one step more for these and drops the penultimate sigma (the samplers minicomfy has)
+DISCARD_PENULTIMATE_SIGMA_SAMPLERS = {"dpm_2"}
 
 
 class KSAMPLER:
@@ -426,10 +454,14 @@ class KSampler:
         self.sampler = sampler
         self.model_options = model_options
         ms = model.model.model_sampling
+        discard = sampler in DISCARD_PENULTIMATE_SIGMA_SAMPLERS
+        n = steps + 1 if discard else steps
         if scheduler == "karras":
-            self.sigmas = get_sigmas_karras(steps, float(ms.sigma_min), float(ms.sigma_max))
+            self.sigmas = get_sigmas_karras(n, float(ms.sigma_min), float(ms.sigma_max))
         else:
-            self.sigmas = simple_scheduler(ms, steps)
+            self.sigmas = simple_scheduler(ms, n)
+        if discard:
+            self.sigmas = torch.cat([self.sigmas[:-2], self.sigmas[-1:]])
         if denoise is not None and denoise < 0.9999 and denoise > 0.0:
             new_steps = int(steps / denoise)
             full = KSampler(model, new_steps, device, sampler, scheduler, None, model_options).sigmas
