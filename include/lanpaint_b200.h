@@ -34,7 +34,7 @@ extern "C" {
 /* Backward-compatible additions within LP_ABI_VERSION: 1 = LP_HEADS_DEAD (a dtype bit every earlier library
  * rejected with LP_ERR_INVALID, so no earlier caller can have set it); 2 = lp_multistep and
  * lp_boundary_multistep (a new entry point: nothing an earlier caller binds changes).  Later entry points
- * (lp_midpoint and lp_boundary_midpoint) leave LP_ABI_MINOR at 2: a caller detects one by its symbol, which is
+ * (lp_midpoint and lp_boundary_midpoint, lp_deis and lp_boundary_deis) leave LP_ABI_MINOR at 2: a caller detects one by its symbol, which is
  * how lanpaint_b200._native binds every entry point (by name). */
 #define LP_ABI_MINOR 2
 #define LP_TABLE_STRIDE 32 /* floats per table row (one 128-byte line), layout below */
@@ -425,6 +425,39 @@ typedef struct lp_midpoint {
 int lp_boundary_midpoint(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                          const lp_known* known, const float* x_in, const float* x_base, float* x_out, float* out,
                          const lp_midpoint* step, const float* next_table, const lp_dims* dims, lp_stream_t stream);
+
+/* One outer step of ComfyUI's sample_deis (DEIS, max_order 3, 'tab' mode): x = x + c_cur*d [+ c_prev1*d_{i-1}
+ * [+ c_prev2*d_{i-2}]] with d = (x - out) / sigma.  The host takes the coefficients from the sampler's own
+ * get_deis_coeff_list (fp32); on a first-order step (the first one, and the step to sigma = 0) c_cur is the fp32
+ * difference sigma_next - sigma and the other two are unused. */
+typedef struct lp_deis {
+  float sigma;   /* the sigma d divides by */
+  float c_cur;   /* weight of this step's derivative */
+  float c_prev1; /* weight of the previous step's (second- and third-order steps) */
+  float c_prev2; /* weight of the one before it (third-order steps) */
+} lp_deis;
+
+/* The boundary of an outer step of a host-owned DEIS loop in ONE pass: lp_boundary_known with the Euler update
+ * replaced by sample_deis's:
+ *   den = model_out->combine ? b + (a - b)*cfg : a
+ *   out = mask ? y : den                                                written when out != NULL
+ *   d   = (x - out) / sigma
+ *   x   = x + c_cur*d                                                   when d_prev1 == NULL (first order)
+ *   x   = x + c_cur*d + c_prev1*d_prev1                                 when d_prev2 == NULL (second order)
+ *   x   = x + c_cur*d + c_prev1*d_prev1 + c_prev2*d_prev2               otherwise (third order)
+ *   d_out = d                                                           written when d_out != NULL
+ *   x   = mask ? rep_noise*noise + rep_y*y : x  (row of next_table)     when next_table != NULL
+ * d_prev1 and d_prev2 are the d_out of the two previous steps.  Every operation of the update is the single correctly
+ * rounded fp32 operation the eager sampler issues (sub, div, mul, add, left to right; never contracted), so x equals
+ * the un-fused route's bit for bit.  d_out is written at every position, known ones included: a later step with no
+ * next_table (the last step of a window that ends above sigma = 0) updates known positions from it.  d_prev1 and
+ * d_prev2 are read only where the update survives (free positions; known positions too when next_table == NULL).
+ * d_prev2 needs d_prev1; d_out, d_prev1 and d_prev2 overlap neither each other nor x_inout or out.  known may be NULL
+ * (dense y / noise / mask). */
+int lp_boundary_deis(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                     const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev1,
+                     const float* d_prev2, const lp_deis* step, const float* next_table, const lp_dims* dims,
+                     lp_stream_t stream);
 
 /* Final denoise of an outer step straight from raw cond / uncond predictions:
  *   out = mask ? y : uncond + (cond - uncond)*cfg ;  if x_inout != NULL: x = x + (x - out)*euler_coef. */

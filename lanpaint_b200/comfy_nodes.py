@@ -24,6 +24,7 @@ nodes exist here: mask/video/audio tooling is outside the hot path (SURVEY 2).
 from __future__ import annotations
 
 import math
+import sys
 from contextlib import contextmanager
 
 import torch
@@ -392,7 +393,8 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         with the option "fused_ancestral" the same holds for euler_ancestral, whose step and randn_like draw
         run inside lp_boundary_ancestral; dpmpp_2m runs there too (on by default), its update and the previous
         step's denoised latent inside lp_boundary_multistep, and so does dpm_2 (on by default), both of its wrapper
-        calls per step in the loop and both of its updates inside lp_boundary_midpoint;
+        calls per step in the loop and both of its updates inside lp_boundary_midpoint, and deis (on by default),
+        its third-order update and the derivatives of the two previous steps inside lp_boundary_deis;
       * any other deterministic sampler: the first job records which sigmas the sampler hands the wrapper, then
         k-diffusion's sampler function itself is captured into ONE graph (`runner.SamplerGraphJob`);
       * anything else (samplers that draw their own noise, early stop, AV packs, mask schedules): k-diffusion's own
@@ -473,6 +475,8 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             fused = dict(sampler="dpmpp_2m")
         elif KSAMPLER._fused_dpm_2_ok(self, model_k, denoise_mask, model_options, engine):
             fused = dict(sampler="dpm_2")
+        elif KSAMPLER._fused_deis_ok(self, model_k, denoise_mask, model_options, engine):
+            fused = dict(sampler="deis", sampler_fn=self.sampler_function)
         elif KSAMPLER._fused_euler_ok(self, model_k, denoise_mask, model_options, engine):
             fused = {}
         if opts.get("fused_sampler", True) and fused is not None:
@@ -571,6 +575,18 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         runner.GraphedJob(sampler="dpm_2"): the sampler without extra options (no churn), and the exclusions of
         `_fused_euler_ok`."""
         if getattr(self.sampler_function, "__name__", "") != "sample_dpm_2" or self.extra_options:
+            return False
+        return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
+
+    def _fused_deis_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
+        """True when ComfyUI's sample_deis around the per-sigma wrapper is the host-owned loop of
+        runner.GraphedJob(sampler="deis"): the sampler without extra options (max_order 3, 'tab' mode), its module's
+        `deis.get_deis_coeff_list` to take the coefficients from, and the exclusions of `_fused_euler_ok`."""
+        fn = self.sampler_function
+        if getattr(fn, "__name__", "") != "sample_deis" or self.extra_options:
+            return False
+        deis = getattr(sys.modules.get(getattr(fn, "__module__", None) or ""), "deis", None)
+        if not callable(getattr(deis, "get_deis_coeff_list", None)):
             return False
         return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
 

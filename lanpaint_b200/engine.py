@@ -534,14 +534,16 @@ class LanPaint:
     def _launch_sequence(self, xm, y, nz, pm, dims, tab, t_model, sigma_dev, cbuf, out, active, plan, call_scaling,
                          model_options, seed, stopper, rng_state, euler_coef=None, skip_prologue=False,
                          next_table=None, current_times=None, ancestral=None, discard_heads=False, multistep=None,
-                         midpoint=None):
+                         midpoint=None, deis=None):
         """discard_heads: the caller owns the network's outputs and nothing reads them once the update kernel that
         consumes them has run (`heads_discardable`), so that kernel may drop them from the L2 unwritten
         (LP_HEADS_DEAD).  Only the fused loop's launches take it; the early-stop loop hands the heads to the stopper.
         multistep: (lp_multistep, the previous step's denoised latent or None): the boundary is
         lp_boundary_multistep, the update of a host-owned sample_dpmpp_2m loop.
         midpoint: (lp_midpoint, x_base, x_out): the boundary is lp_boundary_midpoint, one update of a host-owned
-        sample_dpm_2 loop, with xm -- the state this call's sub-steps ran on -- as its x_in."""
+        sample_dpm_2 loop, with xm -- the state this call's sub-steps ran on -- as its x_in.
+        deis: (lp_deis, d_out, d_prev1, d_prev2), each buffer or None: the boundary is lp_boundary_deis, the update of a
+        host-owned sample_deis loop."""
         lib = _native.load()
         dev = xm.device
         stream = _P(_stream_ptr(dev))
@@ -684,6 +686,16 @@ class LanPaint:
                                           C.byref(step), _P(next_table.data_ptr()) if next_table is not None else None,
                                           C.byref(dims), stream)
             _native.check(rc, "lp_boundary_midpoint")
+            self.launches += 1
+            return done
+        if deis is not None:
+            step, d_out, p1, p2 = deis
+            rc = lib.lp_boundary_deis(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
+                                      C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
+                                      _P(xm.data_ptr()), _P(_ptr(out)), _P(_ptr(d_out)), _P(_ptr(p1)), _P(_ptr(p2)),
+                                      C.byref(step), _P(next_table.data_ptr()) if next_table is not None else None,
+                                      C.byref(dims), stream)
+            _native.check(rc, "lp_boundary_deis")
             self.launches += 1
             return done
         fused_next = next_table is not None and euler_coef is not None

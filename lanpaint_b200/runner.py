@@ -20,7 +20,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _native
-from .schedule import ancestral_step, dpm_2_step, dpmpp_2m_step, effective_inner_steps, times_from_sigma
+from .schedule import ancestral_step, deis_step, dpm_2_step, dpmpp_2m_step, effective_inner_steps, times_from_sigma
 
 
 class VESampling:
@@ -244,6 +244,29 @@ def dpm_2_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask,
     return x
 
 
+def deis_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask, sched: HostSchedule,
+                 sampler_fn) -> torch.Tensor:
+    """`euler_inpaint` with ComfyUI's sample_deis (max_order 3, 'tab') as the sampler: the un-fused definition of
+    GraphedJob(sampler="deis"), eager torch ops around every wrapper call with the coefficients of `sampler_fn`'s own
+    module (`deis_step`) and the derivative d = (x - denoised) / sigma divided by the device schedule's sigma."""
+    dev = latent_image.device
+    sampling = engine.inner_model.inner_model.model_sampling
+    sig = sched.sigmas.to(dev)
+    x = sampling.noise_scaling(sig[0], noise, latent_image)
+    hist = []
+    for i, (st, (_, c_cur, c_prev1, c_prev2, order)) in enumerate(zip(sched.steps, deis_step(sampler_fn, sig))):
+        denoised = engine(x, latent_image, noise, st.sigma_t, mask, st.times, None, 0, n_steps=st.n_inner)
+        d = (x - denoised) / sig[i]
+        t = lambda v: torch.tensor(v, dtype=torch.float32, device=dev)   # noqa: E731
+        x = x + t(c_cur) * d
+        if order >= 2:
+            x = x + t(c_prev1) * hist[-1]
+        if order >= 3:
+            x = x + t(c_prev2) * hist[-2]
+        hist = (hist + [d])[-2:]
+    return x
+
+
 def time_steady_substep(engine, latent_image: torch.Tensor, mask, sigma: float, launches: int = 53,
                         repeats: int = 20, flow: bool = False, rotate: int = 3):
     """Roofline probe: `launches` steady fused sub-step launches (flags = FUSE_NEXT, the kernel that
@@ -329,18 +352,24 @@ class GraphedJob:
     (src/LanPaint/nodes.py:459 "Recommended: euler").
 
     Semantics are exactly `euler_inpaint(engine, ...)`, i.e. k-diffusion's sample_euler around the
-    per-sigma wrapper (asserted bit-for-bit by the tests); sampler="euler_ancestral", "dpmpp_2m" and "dpm_2" are
-    `euler_ancestral_inpaint`, `dpmpp_2m_inpaint` and `dpm_2_inpaint`.  dpm_2 makes two wrapper calls per outer step:
-    call A at sigma_i on x, call B at the midpoint sigma on a second state buffer x2; both are in the step's graph."""
+    per-sigma wrapper (asserted bit-for-bit by the tests); sampler="euler_ancestral", "dpmpp_2m", "dpm_2" and "deis" are
+    `euler_ancestral_inpaint`, `dpmpp_2m_inpaint`, `dpm_2_inpaint` and `deis_inpaint`.  dpm_2 makes two wrapper calls
+    per outer step: call A at sigma_i on x, call B at the midpoint sigma on a second state buffer x2; both are in the
+    step's graph.  deis takes its coefficients from the sampler function `sampler_fn` (ComfyUI's sample_deis or a
+    stand-in with a `deis` module beside it)."""
 
     def __init__(self, engine, sched: HostSchedule, shape, device, flow: bool = False, fused_euler: bool = True,
                  l2_persist: bool = False, model_options=None, seed=0, external_init: bool = False,
-                 first_replace_noop=None, sampler: str = "euler", eta: float = 1.0, s_noise: float = 1.0):
+                 first_replace_noop=None, sampler: str = "euler", eta: float = 1.0, s_noise: float = 1.0,
+                 sampler_fn=None):
         import numpy as np
         from .engine import _DrawPlan
-        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m", "dpm_2"):
-            raise ValueError("GraphedJob owns the loops of 'euler', 'euler_ancestral', 'dpmpp_2m' and 'dpm_2', "
+        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m", "dpm_2", "deis"):
+            raise ValueError("GraphedJob owns the loops of 'euler', 'euler_ancestral', 'dpmpp_2m', 'dpm_2' and 'deis', "
                              f"not {sampler!r}")
+        if sampler == "deis" and sampler_fn is None:
+            raise ValueError("GraphedJob(sampler='deis') needs the sampler function (sampler_fn): the coefficients are "
+                             "its module's")
         self.sampler = sampler
         self.fused_euler = fused_euler   # the sampler's update inside the step-boundary kernel instead of torch kernels
         # optional persisting-L2 window over the clean latent (re-read by every launch).  Off by default: the
@@ -424,6 +453,16 @@ class GraphedJob:
                                                for st, (a, b, _) in zip(sched.steps, self.midpoint)],
                                               dtype=torch.float32, device=dev)
             self.out_mid = mk() if not fused_euler else None   # the midpoint call's denoised latent (un-fused update)
+        # deis: per outer step (lp_deis, order, whether a later step reads its derivative), the coefficients read back
+        # once here, and a ring of three derivative buffers: step i writes d_ring[i % 3] and reads the two before it,
+        # so every per-step graph bakes in a fixed triple.  No draw of its own
+        self.deis = self.d_ring = None
+        if sampler == "deis":
+            rows = deis_step(sampler_fn, sched.sigmas)
+            self.deis = [(_native.Deis(sigma, c_cur, c_prev1, c_prev2), order, i + 1 < len(rows) and rows[i + 1][4] >= 2)
+                         for i, (sigma, c_cur, c_prev1, c_prev2, order) in enumerate(rows)]
+            self.d_ring = (mk(), mk(), mk())
+            self.deis_scalars = torch.tensor([r[:4] for r in rows], dtype=torch.float32, device=dev)
         draws = lambda n: 0 if n <= 0 else (n if merged else 2 * n - 1)   # noqa: E731  one wrapper call's draws
         self._call_draws = draws
         self.draws_before = [0]
@@ -481,10 +520,15 @@ class GraphedJob:
         st = self.sched.steps[i]
         coef = (st.sigma_next - st.sigma) / st.sigma
         anc = self.ancestral[i] if self.ancestral is not None else None
-        ms, old = None, None
+        ms, old, dz = None, None, None
         if self.multistep is not None:
             ms = self.multistep[i]
             old = self.denoised_buffer(i - 1, want_out) if ms[1] else None
+        if self.deis is not None:     # (lp_deis, d_out, d_prev1, d_prev2)
+            step, order, keep = self.deis[i]
+            ring = self.d_ring
+            dz = (step, ring[i % 3] if keep else None, ring[(i - 1) % 3] if order >= 2 else None,
+                  ring[(i - 2) % 3] if order >= 3 else None)
         last = i + 1 == len(self.sched.steps)
         plan.used = self.draws_before[i]
         out = self.out if (want_out or not self.fused_euler) else None
@@ -495,12 +539,25 @@ class GraphedJob:
         eng._launch_sequence(self.x, self.y, self.noise, self.mask, self._dims, self.tables[i], self.t_model[i],
                              self.sigma[i], self.c, out, self.active[i], plan, False, self.model_options, self.seed,
                              None, self.rng_state.data_ptr(), discard_heads=heads_discardable(self.model_options),
-                             euler_coef=coef if (self.fused_euler and anc is None and ms is None) else None,
+                             euler_coef=coef if (self.fused_euler and anc is None and ms is None and dz is None) else None,
                              skip_prologue=(self.fused_euler and i > 0) or (i == 0 and self.first_replace_noop),
                              next_table=self.tables[i + 1] if (self.fused_euler and not last) else None,
                              ancestral=anc if self.fused_euler else None,
-                             multistep=(ms[0], old) if (self.fused_euler and ms is not None) else None)
+                             multistep=(ms[0], old) if (self.fused_euler and ms is not None) else None,
+                             deis=dz if self.fused_euler else None)
         if self.fused_euler:
+            return
+        if dz is not None:     # sample_deis's tensor ops, in its order
+            sc = self.deis_scalars[i]
+            d = (self.x - out) / sc[0]
+            x = self.x + sc[1] * d
+            if dz[2] is not None:
+                x = x + sc[2] * dz[2]
+            if dz[3] is not None:
+                x = x + sc[3] * dz[3]
+            self.x.copy_(x)
+            if dz[1] is not None:
+                dz[1].copy_(d)
             return
         # un-fused: from this step's denoised latent, wherever it was written
         if ms is not None:     # sample_dpmpp_2m's tensor ops, in its order
@@ -712,7 +769,7 @@ class SamplerGraphJob:
     """ANY deterministic k-diffusion sampler around the per-sigma wrapper as ONE CUDA graph per job.
 
     `runner.GraphedJob` owns the sampler loop, so it only serves the samplers it restates (euler, euler_ancestral,
-    dpmpp_2m, dpm_2).  For the other samplers (heun, deis, res_multistep, ...) the loop is third-party Python that
+    dpmpp_2m, dpm_2, deis).  For the other samplers (heun, res_multistep, ...) the loop is third-party Python that
     calls the wrapper with sigma values only it knows.  But for a fixed schedule that sequence is deterministic: the node layer records it during the first,
     eager job of a configuration (`KSamplerX0Inpaint.trace`), this class turns every recorded call into device
     constants (`engine.plan_item`) and then runs the sampler function ITSELF under stream capture -- its Python runs

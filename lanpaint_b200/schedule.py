@@ -119,6 +119,29 @@ def dpm_2_step(sigmas: torch.Tensor):
     return [(v[0], v[1], v[2], host[i + 1] != 0.0) for i, v in enumerate(vals)]
 
 
+def deis_step(sampler_fn, sigmas: torch.Tensor):
+    """[(sigma, c_cur, c_prev1, c_prev2, order)] for every outer step of ComfyUI's sample_deis (max_order = 3,
+    deis_mode = 'tab') on `sigmas`: x = x + c_cur d [+ c_prev1 d_{i-1} [+ c_prev2 d_{i-2}]], d = (x - denoised) / sigma.
+
+    The coefficients are the sampler's own: `get_deis_coeff_list` of the `deis` module next to `sampler_fn` (ComfyUI's
+    k_diffusion.sampling, or the stand-in), 0-d fp32 CPU tensors, called once here (it runs autograd on the CPU).
+    order = min(3, i + 1), and 1 on the step to sigma <= 0; a first-order step's c_cur is the sampler's fp32
+    difference sigma_next - sigma of schedule entries, evaluated where `sigmas` lives.  Unused coefficients are 0."""
+    import sys
+    deis = sys.modules[sampler_fn.__module__].deis
+    with torch.no_grad():
+        coeff = deis.get_deis_coeff_list(sigmas, 3, deis_mode="tab")
+        host = [float(v) for v in sigmas.detach().cpu()]
+        first = (sigmas[1:] - sigmas[:-1]).to(torch.float32).cpu().tolist()
+    rows = []
+    for i in range(len(host) - 1):
+        order = 1 if host[i + 1] <= 0 else min(3, i + 1)
+        c = [first[i]] if order == 1 else [float(v.to(torch.float32)) for v in coeff[i][:order]]
+        c += [0.0] * (3 - len(c))
+        rows.append((host[i], c[0], c[1], c[2], order))
+    return rows
+
+
 @dataclass
 class Hyper:
     step_size: float

@@ -21,6 +21,8 @@ from typing import Callable
 
 import torch
 
+from . import deis  # noqa: F401  sample_deis reads its coefficients through this attribute, as ComfyUI's does
+
 
 # ------------------------------------------------------------------ model side
 class ModelType:
@@ -322,8 +324,49 @@ def sample_dpm_2(model, x, sigmas, extra_args=None, callback=None, disable=None)
     return x
 
 
+@torch.no_grad()
+def sample_deis(model, x, sigmas, extra_args=None, callback=None, disable=None, max_order=3, deis_mode="tab"):
+    """ComfyUI's DEIS sampler: a multistep update from this step's derivative and the last max_order - 1 ones, with
+    the coefficients of `deis.get_deis_coeff_list`; first order on the first step and on the step to sigma = 0.
+    As ComfyUI's, its callback sees the sampler's initial x."""
+    extra_args = extra_args or {}
+    s_in = x.new_ones([x.shape[0]])
+    x_next = x
+    coeff_list = deis.get_deis_coeff_list(sigmas, max_order, deis_mode=deis_mode)
+    buffer_model = []
+    for i in range(len(sigmas) - 1):
+        t_cur, t_next = sigmas[i], sigmas[i + 1]
+        x_cur = x_next
+        denoised = model(x_cur, t_cur * s_in, **extra_args)
+        if callback is not None:
+            callback({"x": x, "i": i, "sigma": sigmas[i], "sigma_hat": sigmas[i], "denoised": denoised})
+        d_cur = (x_cur - denoised) / t_cur
+        order = min(max_order, i + 1)
+        if t_next <= 0:
+            order = 1
+        if order == 1:
+            x_next = x_cur + (t_next - t_cur) * d_cur
+        elif order == 2:
+            coeff_cur, coeff_prev1 = coeff_list[i]
+            x_next = x_cur + coeff_cur * d_cur + coeff_prev1 * buffer_model[-1]
+        elif order == 3:
+            coeff_cur, coeff_prev1, coeff_prev2 = coeff_list[i]
+            x_next = x_cur + coeff_cur * d_cur + coeff_prev1 * buffer_model[-1] + coeff_prev2 * buffer_model[-2]
+        else:
+            coeff_cur, coeff_prev1, coeff_prev2, coeff_prev3 = coeff_list[i]
+            x_next = (x_cur + coeff_cur * d_cur + coeff_prev1 * buffer_model[-1] + coeff_prev2 * buffer_model[-2]
+                      + coeff_prev3 * buffer_model[-3])
+        if len(buffer_model) == max_order - 1:
+            for k in range(max_order - 2):
+                buffer_model[k] = buffer_model[k + 1]
+            buffer_model[-1] = d_cur.detach()
+        else:
+            buffer_model.append(d_cur.detach())
+    return x_next
+
+
 _SAMPLER_FUNCTIONS = {"euler": sample_euler, "heun": sample_heun, "euler_ancestral": sample_euler_ancestral,
-                      "dpmpp_2m": sample_dpmpp_2m, "dpm_2": sample_dpm_2}
+                      "dpmpp_2m": sample_dpmpp_2m, "dpm_2": sample_dpm_2, "deis": sample_deis}
 # ComfyUI's KSampler takes one step more for these and drops the penultimate sigma (the samplers minicomfy has)
 DISCARD_PENULTIMATE_SIGMA_SAMPLERS = {"dpm_2"}
 
