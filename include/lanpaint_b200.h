@@ -34,7 +34,8 @@ extern "C" {
 /* Backward-compatible additions within LP_ABI_VERSION: 1 = LP_HEADS_DEAD (a dtype bit every earlier library
  * rejected with LP_ERR_INVALID, so no earlier caller can have set it); 2 = lp_multistep and
  * lp_boundary_multistep (a new entry point: nothing an earlier caller binds changes).  Later entry points
- * (lp_midpoint and lp_boundary_midpoint, lp_deis and lp_boundary_deis) leave LP_ABI_MINOR at 2: a caller detects one by its symbol, which is
+ * (lp_midpoint and lp_boundary_midpoint, lp_deis and lp_boundary_deis, lp_gradient_estimation and
+ * lp_boundary_gradient_estimation) leave LP_ABI_MINOR at 2: a caller detects one by its symbol, which is
  * how lanpaint_b200._native binds every entry point (by name). */
 #define LP_ABI_MINOR 2
 #define LP_TABLE_STRIDE 32 /* floats per table row (one 128-byte line), layout below */
@@ -394,7 +395,12 @@ typedef struct lp_multistep {
  * to sigma = 0: the caller passes old_out == NULL exactly then.  Every operation of the update is the single
  * correctly rounded fp32 operation the eager sampler issues (mul, sub; never contracted), so x equals the un-fused
  * route's bit for bit.  old_out is read only where the update survives (free positions; known positions too when
- * next_table == NULL) and must not overlap x_inout or out.  known may be NULL (dense y / noise / mask). */
+ * next_table == NULL) and must not overlap x_inout or out.  known may be NULL (dense y / noise / mask).
+ *
+ * The second-order step of ComfyUI's res_multistep (eta = 0), x = sigma_fn(h)*x + h*(b1*out + b2*old_out), is this
+ * launch with ratio = sigma_fn(h), em1 = -h, c_cur = b1 and c_old = -b2, bit for bit: negation is exact, and IEEE 754
+ * defines a - b as a + (-b), so c_cur*out - c_old*old_out = b1*out + b2*old_out and ratio*x - em1*s = ratio*x + h*s,
+ * each product and sum the same single correctly rounded operation the sampler issues. */
 int lp_boundary_multistep(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                           const lp_known* known, float* x_inout, float* out, const float* old_out,
                           const lp_multistep* step, const float* next_table, const lp_dims* dims, lp_stream_t stream);
@@ -458,6 +464,38 @@ int lp_boundary_deis(const lp_heads* model_out, const float* y, const float* noi
                      const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev1,
                      const float* d_prev2, const lp_deis* step, const float* next_table, const lp_dims* dims,
                      lp_stream_t stream);
+
+/* One outer step of ComfyUI's sample_gradient_estimation (ge_gamma, no cfg_pp): the Euler step x = x + d*dt and,
+ * from the second step on, the gradient-estimation correction x = x + (gm1*(d - d_prev))*dt, with d = (x - out) / sigma;
+ * the step to sigma = 0 is x = out.  The host evaluates sigma and dt with the sampler's own torch expressions on the
+ * schedule, on the device the sampler runs on, and reads them back; gm1 is the fp32 value of ge_gamma - 1. */
+typedef struct lp_gradient_estimation {
+  float sigma; /* sigma_i, the sigma d divides by */
+  float dt;    /* sigma_next - sigma_i */
+  float gm1;   /* ge_gamma - 1 */
+  int final;   /* nonzero on the step to sigma = 0: x = out */
+} lp_gradient_estimation;
+
+/* The boundary of an outer step of a host-owned gradient-estimation loop in ONE pass: lp_boundary_known with the Euler
+ * update replaced by sample_gradient_estimation's:
+ *   den   = model_out->combine ? b + (a - b)*cfg : a
+ *   out   = mask ? y : den                                              written when out != NULL
+ *   d     = (x - out) / sigma
+ *   x     = out                                                         when step->final (the sampler's x = denoised)
+ *   x     = x + d*dt                                                    otherwise
+ *   x     = x + (gm1*(d - d_prev))*dt                                   when d_prev != NULL (after the line above)
+ *   d_out = d                                                           when d_out != NULL, at every position
+ *   x     = mask ? rep_noise*noise + rep_y*y : x  (row of next_table)   when next_table != NULL
+ * d_prev is the previous step's d_out.  Every operation of the update is the single correctly rounded fp32 operation
+ * the eager sampler issues (sub, div, mul, add in its order; never contracted), so x equals the un-fused route's bit
+ * for bit.  d_out is written at every position, known ones included: a later step with no next_table (the last step of
+ * a window that ends above sigma = 0) updates known positions from it.  d_prev is read only where the update survives
+ * (free positions; known positions too when next_table == NULL).  final excludes d_prev; d_out, d_prev, x_inout and
+ * out overlap none of each other.  known may be NULL (dense y / noise / mask). */
+int lp_boundary_gradient_estimation(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                                    const lp_known* known, float* x_inout, float* out, float* d_out,
+                                    const float* d_prev, const lp_gradient_estimation* step, const float* next_table,
+                                    const lp_dims* dims, lp_stream_t stream);
 
 /* Final denoise of an outer step straight from raw cond / uncond predictions:
  *   out = mask ? y : uncond + (cond - uncond)*cfg ;  if x_inout != NULL: x = x + (x - out)*euler_coef. */

@@ -393,8 +393,12 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         with the option "fused_ancestral" the same holds for euler_ancestral, whose step and randn_like draw
         run inside lp_boundary_ancestral; dpmpp_2m runs there too (on by default), its update and the previous
         step's denoised latent inside lp_boundary_multistep, and so does dpm_2 (on by default), both of its wrapper
-        calls per step in the loop and both of its updates inside lp_boundary_midpoint, and deis (on by default),
-        its third-order update and the derivatives of the two previous steps inside lp_boundary_deis;
+        calls per step in the loop and both of its updates inside lp_boundary_midpoint, deis (on by default),
+        its third-order update and the derivatives of the two previous steps inside lp_boundary_deis,
+        res_multistep (on by default when extra_args has a seed), its second-order step inside lp_boundary_multistep
+        and its Euler steps inside lp_boundary_midpoint, and gradient_estimation (on by default), its update and
+        the previous step's derivative inside lp_boundary_gradient_estimation; each of the last two only when a
+        check of the sampler function on a tiny CPU problem shows the form the loop restates;
       * any other deterministic sampler: the first job records which sigmas the sampler hands the wrapper, then
         k-diffusion's sampler function itself is captured into ONE graph (`runner.SamplerGraphJob`);
       * anything else (samplers that draw their own noise, early stop, AV packs, mask schedules): k-diffusion's own
@@ -477,6 +481,10 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             fused = dict(sampler="dpm_2")
         elif KSAMPLER._fused_deis_ok(self, model_k, denoise_mask, model_options, engine):
             fused = dict(sampler="deis", sampler_fn=self.sampler_function)
+        elif KSAMPLER._fused_res_multistep_ok(self, model_k, denoise_mask, model_options, engine, extra_args):
+            fused = dict(sampler="res_multistep")
+        elif KSAMPLER._fused_gradient_estimation_ok(self, model_k, denoise_mask, model_options, engine):
+            fused = dict(sampler="gradient_estimation")
         elif KSAMPLER._fused_euler_ok(self, model_k, denoise_mask, model_options, engine):
             fused = {}
         if opts.get("fused_sampler", True) and fused is not None:
@@ -589,6 +597,30 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         if not callable(getattr(deis, "get_deis_coeff_list", None)):
             return False
         return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
+
+    def _fused_res_multistep_ok(self, model_k, denoise_mask, model_options, engine, extra_args) -> bool:
+        """True when ComfyUI's sample_res_multistep around the per-sigma wrapper is the host-owned loop of
+        runner.GraphedJob(sampler="res_multistep"): the sampler without extra options (eta = 0), a seed in extra_args
+        (its draw, multiplied by sigma_up = 0, then comes from a private generator, so skipping it leaves every
+        generator as the sampler leaves it), the exclusions of `_fused_euler_ok`, and the form check of
+        `_restates`."""
+        fn = self.sampler_function
+        if getattr(fn, "__name__", "") != "sample_res_multistep" or self.extra_options:
+            return False
+        if (extra_args or {}).get("seed") is None:
+            return False
+        return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine) and _restates(fn, "res_multistep")
+
+    def _fused_gradient_estimation_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
+        """True when ComfyUI's sample_gradient_estimation around the per-sigma wrapper is the host-owned loop of
+        runner.GraphedJob(sampler="gradient_estimation"): the sampler without extra options (ge_gamma = 2), the
+        exclusions of `_fused_euler_ok`, and the form check of `_restates` (ComfyUI has shipped an older form that
+        the loop does not restate)."""
+        fn = self.sampler_function
+        if getattr(fn, "__name__", "") != "sample_gradient_estimation" or self.extra_options:
+            return False
+        return (KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
+                and _restates(fn, "gradient_estimation"))
 
     def _fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options, seed, flow,
                      early_stop, callback, total_steps, use_graph, opts, sampler=None):
@@ -716,6 +748,69 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         entry.runs += 1
         LAST_RUN.update(mode="sampler-graph", fused=False, job=job)
         return out if out.dtype == x_init.dtype else out.to(x_init.dtype)
+
+
+# =============================================================================================
+# the form check of the res_multistep and gradient_estimation gates
+# =============================================================================================
+def _res_multistep_form(model, x, sigmas):
+    """runner.GraphedJob(sampler="res_multistep")'s update from `res_multistep_step`'s scalars, in x's dtype."""
+    from .schedule import res_multistep_step
+    old = None
+    for i, (second, a, b, c, e) in enumerate(res_multistep_step(sigmas.to(torch.float32))):
+        den = model(x, sigmas[i])
+        x = a * x - b * (c * den - e * old) if second else x + ((x - den) / a) * b
+        old = den
+    return x
+
+
+def _gradient_estimation_form(model, x, sigmas):
+    """runner.GraphedJob(sampler="gradient_estimation")'s update from `gradient_estimation_step`'s scalars, in x's
+    dtype."""
+    from .schedule import gradient_estimation_step
+    old = None
+    for i, (sigma, dt, gm1, reads, final, _) in enumerate(gradient_estimation_step(sigmas.to(torch.float32))):
+        den = model(x, sigmas[i])
+        d = (x - den) / sigma
+        if final:
+            x = den
+        else:
+            x = x + d * dt
+            if reads:
+                x = x + gm1 * (d - old) * dt
+        old = d
+    return x
+
+
+_FORMS = {"res_multistep": _res_multistep_form, "gradient_estimation": _gradient_estimation_form}
+_FORM_OK = {}     # (sampler function, sampler) -> whether the function computes the form of that fused loop
+
+
+def _restates(fn, sampler: str) -> bool:
+    """Whether the sampler function `fn` computes what the fused loop of `sampler` restates: `fn` runs once, in fp64
+    on the CPU, around an affine stand-in network, on a 5-step schedule that ends at 0 and on a window that ends above
+    it, and its results must match the loop's update from its own fp32 scalars to 1e-5.  Cached per function."""
+    key = (fn, sampler)
+    ok = _FORM_OK.get(key)
+    if ok is None:
+        g = torch.Generator().manual_seed(0)
+        x0 = torch.randn(2, 3, 4, 4, generator=g, dtype=torch.float64) * 5
+        bias = torch.randn(2, 3, 4, 4, generator=g, dtype=torch.float64)
+        model = lambda x, sigma, **kw: 0.75 * x + 0.25 * bias   # noqa: E731
+        ok = True
+        for sig in ([5.0, 2.5, 1.1, 0.4, 0.1, 0.0], [5.0, 2.5, 1.1, 0.4]):
+            sigmas = torch.tensor(sig, dtype=torch.float64)
+            try:
+                got = fn(model, x0.clone(), sigmas, extra_args={"seed": 0}, callback=None, disable=True)
+            except Exception:
+                ok = False
+                break
+            want = _FORMS[sampler](model, x0.clone(), sigmas)
+            if not float((got - want).abs().max()) <= 1e-5 * float(want.abs().max()):
+                ok = False
+                break
+        _FORM_OK[key] = ok
+    return ok
 
 
 # =============================================================================================

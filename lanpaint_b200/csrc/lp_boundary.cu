@@ -10,6 +10,7 @@
 //                       the same boundary for either wrapper call of k-diffusion's sample_dpm_2 (DPM-Solver-2)
 //   boundary_deis_kernel
 //                       the same boundary for ComfyUI's sample_deis (DEIS, third order), writing the step's derivative
+//   boundary_ge_kernel  the same boundary for ComfyUI's sample_gradient_estimation, writing the step's derivative
 //   advance_kernel      one un-fused advance_time_overdamped             lanpaint.py:232-254
 //   stop_stats_kernel   early-stop masked reductions                     earlystop.py:32-55,238-313
 #include "lp_common.cuh"
@@ -1269,6 +1270,164 @@ static int boundary_deis_impl(const lp_heads* mo, const float* y, const float* n
   }
 }
 
+// ---- the boundary of an outer step of a host-owned gradient-estimation loop ---------------------------------------
+// ComfyUI's sample_gradient_estimation issues, after the wrapper call, sub, div, then mul, add (the Euler step) and,
+// from its second step on, sub, mul, mul, add (the correction), with scalars the host hands in as
+// lp_gradient_estimation; lp_boundary_gradient_estimation does them in the boundary's one pass, each as the same
+// correctly rounded fp32 operation, and keeps d for the next step.
+struct GeArgs {
+  BoundaryArgs b;      // x is never NULL; coef is unused
+  lp_gradient_estimation st;
+  float* dout;         // NULL: no later step reads this step's d
+  const float* prev;   // the previous step's d; NULL: no correction
+};
+
+// per element: den = combine ? b + (a-b) cfg : a ; o = known ? y : den ; d = (x - o) / sigma ;
+// x = final ? o : x + d dt [+ (gm1 (d - prev)) dt] ; x = known ? rn n + ry y : x
+__device__ __forceinline__ void ge_element(float a, float b, float y, float nz, float pv, bool known, float& x,
+                                           float& o, float& d, bool combine, float cfg,
+                                           const lp_gradient_estimation& st, bool fin, bool hist, bool next, float rn,
+                                           float ry) {
+  const float den = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
+  o = known ? y : den;
+  d = __fdiv_rn(__fsub_rn(x, o), st.sigma);
+  float u = o;
+  if (!fin) {
+    u = __fadd_rn(x, __fmul_rn(d, st.dt));
+    if (hist) u = __fadd_rn(u, __fmul_rn(__fmul_rn(st.gm1, __fsub_rn(d, pv)), st.dt));
+  }
+  x = next && known ? fmaf(rn, nz, ry * y) : u;  // the replace step rounds as prologue_kernel does
+}
+
+// boundary_kernel's form and operand skipping; the history is read where x's update survives, x where the update
+// reads it or d is written
+template <int N, typename H, bool kPk>
+__global__ void __launch_bounds__(kBlock) boundary_ge_kernel(const GeArgs q) {
+  pdl_prologue();
+  const BoundaryArgs& p = q.b;
+  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= p.g.total) return;
+  const uint64_t dead = l2_policy_dead(p.l2);
+  uint32_t row, mi;
+  locate(p.g, i, row, mi);
+  const bool next = p.next_table != nullptr, hist = q.prev != nullptr, fin = q.st.final != 0;
+  float av[N], bv[N], yv[N], xv[N], nv[N], pv[N], ov[N], dv[N];
+  bool known[N];
+  uint32_t kb = 0, kidx = 0;
+  if constexpr (kPk) {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
+    if constexpr (N == 4) {
+      known_quad(w, i, kb, kidx);
+    } else {
+      kb = (w.x >> (i & 31u)) & 1u;
+      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
+    }
+#pragma unroll
+    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
+  } else {
+    load_m<N>(p.mask, mi, known);
+  }
+  bool any_known = false, any_free = false;
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    any_known |= known[j];
+    any_free |= !known[j];
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = pv[j] = 0.f;
+  if constexpr (kPk) {
+    if constexpr (N == 4) {
+      gather_known4<false>(p.yk, kb, kidx, yv);
+    } else {
+      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
+    }
+  } else {
+    load_f_ro<N>(p.y, i, yv);
+  }
+  if (any_free) {
+    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
+    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
+  }
+  const bool update = any_free || !next;  // somewhere in the vector x's update is not overwritten by the replace step
+  if ((update && !fin) || q.dout) load_f<N>(p.x, i, xv);
+  if (hist && update) load_head_ro<N, float>(q.prev, i, pv, dead);  // nothing reads it again
+  float rn = 0.f, ry = 0.f;
+  if (next) {
+    if constexpr (kPk) {
+      if constexpr (N == 4) {
+        gather_known4<false>(p.nk, kb, kidx, nv);
+      } else {
+        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
+      }
+    } else {
+      if (any_known) load_f_ro<N>(p.noise, i, nv);
+    }
+    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
+    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j)
+    ge_element(av[j], bv[j], yv[j], nv[j], pv[j], known[j], xv[j], ov[j], dv[j], p.combine != 0, p.cfg, q.st, fin,
+               hist, next, rn, ry);
+  if (p.out) store_f<N>(p.out, i, ov, dead);
+  if (q.dout) store_f<N>(q.dout, i, dv);  // normal policy: the next step reads it
+  store_f<N>(p.x, i, xv);
+  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
+    if (p.discard) {
+      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
+      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
+        __syncwarp();           // every lane's head loads are used
+        discard_line<H>(p.a, i, end);
+        if (p.b) discard_line<H>(p.b, i, end);
+      }
+    }
+  }
+}
+
+template <typename H>
+int ge_dispatch(const GeArgs& q, bool v4, cudaStream_t s) {
+  const uint32_t total = q.b.g.total;
+  if (q.b.kwords) {
+    if (v4) launch_kernel(boundary_ge_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_ge_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
+  } else {
+    if (v4) launch_kernel(boundary_ge_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_ge_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
+  }
+  return check_launch();
+}
+
+static int boundary_ge_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                            const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev,
+                            const lp_gradient_estimation* step, const float* next_table, const lp_dims* dims,
+                            lp_stream_t stream) {
+  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
+  if (!x_inout || !step || (step->final && d_prev)) return LP_ERR_INVALID;
+  GeArgs q;
+  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  // the launch writes x, out and d_out while it reads d_prev: the four share no byte
+  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
+  const auto any = [&](const void* u, const void* v) { return u && v && (u == v || overlaps(u, v, bytes)); };
+  const void* bufs[4] = {x_inout, out, d_out, d_prev};
+  for (int k = 0; k < 4; ++k)
+    for (int l = 0; l < k; ++l)
+      if (any(bufs[k], bufs[l])) return LP_ERR_INVALID;
+  if (q.b.g.total == 0) return LP_OK;
+  boundary_args(q.b, mo, y, noise, mask, known, x_inout, out, 0.f, next_table);
+  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x_inout, out, d_out, d_prev});  // no state dropped
+  q.st = *step;
+  q.dout = d_out;
+  q.prev = d_prev;
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
+  const bool v4 = boundary_vec4(q.b, dtype) && (!d_out || aligned16(d_out)) && (!d_prev || aligned16(d_prev));
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (dtype) {
+    case LP_DTYPE_F32: return ge_dispatch<float>(q, v4, s);
+    case LP_DTYPE_BF16: return ge_dispatch<__nv_bfloat16>(q, v4, s);
+    default: return ge_dispatch<__half>(q, v4, s);
+  }
+}
+
 // ---- un-fused OU advance (advance_time_overdamped, lanpaint.py:232-254) --------
 struct AdvanceArgs {
   float* x;
@@ -1464,6 +1623,14 @@ extern "C" int lp_boundary_deis(const lp_heads* model_out, const float* y, const
                                 lp_stream_t stream) {
   return boundary_deis_impl(model_out, y, noise, mask, known, x_inout, out, d_out, d_prev1, d_prev2, step, next_table,
                             dims, stream);
+}
+
+extern "C" int lp_boundary_gradient_estimation(const lp_heads* model_out, const float* y, const float* noise,
+                                               const uint8_t* mask, const lp_known* known, float* x_inout, float* out,
+                                               float* d_out, const float* d_prev, const lp_gradient_estimation* step,
+                                               const float* next_table, const lp_dims* dims, lp_stream_t stream) {
+  return boundary_ge_impl(model_out, y, noise, mask, known, x_inout, out, d_out, d_prev, step, next_table, dims,
+                          stream);
 }
 
 extern "C" int lp_epilogue_f32(const float* model_out, const float* y, const uint8_t* mask, float* out,

@@ -20,7 +20,8 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _native
-from .schedule import ancestral_step, deis_step, dpm_2_step, dpmpp_2m_step, effective_inner_steps, times_from_sigma
+from .schedule import (ancestral_step, deis_step, dpm_2_step, dpmpp_2m_step, effective_inner_steps,
+                       gradient_estimation_step, res_multistep_step, times_from_sigma)
 
 
 class VESampling:
@@ -267,6 +268,50 @@ def deis_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask, 
     return x
 
 
+def res_multistep_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask,
+                          sched: HostSchedule) -> torch.Tensor:
+    """`euler_inpaint` with ComfyUI's sample_res_multistep (eta = 0) as the sampler: the un-fused definition of
+    GraphedJob(sampler="res_multistep"), eager torch ops around every wrapper call with the sampler's own scalars
+    (`res_multistep_step` on the schedule, on the latent's device).  The sampler's draw, multiplied by sigma_up = 0,
+    adds a signed zero to every element and is not taken."""
+    dev = latent_image.device
+    sampling = engine.inner_model.inner_model.model_sampling
+    x = sampling.noise_scaling(sched.sigmas[0].to(dev), noise, latent_image)
+    t = lambda v: torch.tensor(v, dtype=torch.float32, device=dev)   # noqa: E731
+    old = None
+    for st, (second, a, b, c, e) in zip(sched.steps, res_multistep_step(sched.sigmas.to(dev))):
+        denoised = engine(x, latent_image, noise, st.sigma_t, mask, st.times, None, 0, n_steps=st.n_inner)
+        if second:     # a, b, c, e = sigma_fn(h), -h, b1, -b2
+            x = t(a) * x + t(-b) * (t(c) * denoised + t(-e) * old)
+        else:          # a, b = sigma_i, sigma_next - sigma_i
+            x = x + ((x - denoised) / t(a)) * t(b)
+        old = denoised
+    return x
+
+
+def gradient_estimation_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask,
+                                sched: HostSchedule) -> torch.Tensor:
+    """`euler_inpaint` with ComfyUI's sample_gradient_estimation (ge_gamma = 2) as the sampler: the un-fused definition
+    of GraphedJob(sampler="gradient_estimation"), eager torch ops around every wrapper call with the sampler's own
+    scalars (`gradient_estimation_step` on the schedule, on the latent's device)."""
+    dev = latent_image.device
+    sampling = engine.inner_model.inner_model.model_sampling
+    x = sampling.noise_scaling(sched.sigmas[0].to(dev), noise, latent_image)
+    t = lambda v: torch.tensor(v, dtype=torch.float32, device=dev)   # noqa: E731
+    old_d = None
+    for st, (sigma, dt, gm1, reads, final, _) in zip(sched.steps, gradient_estimation_step(sched.sigmas.to(dev))):
+        denoised = engine(x, latent_image, noise, st.sigma_t, mask, st.times, None, 0, n_steps=st.n_inner)
+        d = (x - denoised) / t(sigma)
+        if final:
+            x = denoised
+        else:
+            x = x + d * t(dt)
+            if reads:
+                x = x + (gm1 * (d - old_d)) * t(dt)
+        old_d = d
+    return x
+
+
 def time_steady_substep(engine, latent_image: torch.Tensor, mask, sigma: float, launches: int = 53,
                         repeats: int = 20, flow: bool = False, rotate: int = 3):
     """Roofline probe: `launches` steady fused sub-step launches (flags = FUSE_NEXT, the kernel that
@@ -356,7 +401,8 @@ class GraphedJob:
     `euler_ancestral_inpaint`, `dpmpp_2m_inpaint`, `dpm_2_inpaint` and `deis_inpaint`.  dpm_2 makes two wrapper calls
     per outer step: call A at sigma_i on x, call B at the midpoint sigma on a second state buffer x2; both are in the
     step's graph.  deis takes its coefficients from the sampler function `sampler_fn` (ComfyUI's sample_deis or a
-    stand-in with a `deis` module beside it)."""
+    stand-in with a `deis` module beside it).  sampler="res_multistep" (eta = 0) and "gradient_estimation" (ge_gamma =
+    2) are `res_multistep_inpaint` and `gradient_estimation_inpaint`."""
 
     def __init__(self, engine, sched: HostSchedule, shape, device, flow: bool = False, fused_euler: bool = True,
                  l2_persist: bool = False, model_options=None, seed=0, external_init: bool = False,
@@ -364,9 +410,10 @@ class GraphedJob:
                  sampler_fn=None):
         import numpy as np
         from .engine import _DrawPlan
-        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m", "dpm_2", "deis"):
-            raise ValueError("GraphedJob owns the loops of 'euler', 'euler_ancestral', 'dpmpp_2m', 'dpm_2' and 'deis', "
-                             f"not {sampler!r}")
+        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m", "dpm_2", "deis", "res_multistep",
+                           "gradient_estimation"):
+            raise ValueError("GraphedJob owns the loops of 'euler', 'euler_ancestral', 'dpmpp_2m', 'dpm_2', 'deis', "
+                             f"'res_multistep' and 'gradient_estimation', not {sampler!r}")
         if sampler == "deis" and sampler_fn is None:
             raise ValueError("GraphedJob(sampler='deis') needs the sampler function (sampler_fn): the coefficients are "
                              "its module's")
@@ -389,7 +436,7 @@ class GraphedJob:
         mk = lambda: torch.empty(self.shape, dtype=torch.float32, device=dev)
         self.x, self.y, self.noise, self.c, self.out = mk(), mk(), mk(), mk(), mk()
         # dpmpp_2m writes every step's denoised latent and reads it back at the next step: two buffers taken in turn
-        self.out_pair = (self.out, mk()) if sampler == "dpmpp_2m" else None
+        self.out_pair = (self.out, mk()) if sampler in ("dpmpp_2m", "res_multistep") else None
         # dpm_2: the midpoint call's state (x_2 of the sampler)
         self.x2 = mk() if sampler == "dpm_2" else None
         self.mask = None
@@ -430,6 +477,14 @@ class GraphedJob:
         if sampler == "dpmpp_2m":
             self.multistep = [(_native.Multistep(ratio, em1, c_cur, c_old), second)
                               for ratio, em1, c_cur, c_old, second in dpmpp_2m_step(sched.sigmas.to(dev))]
+        # res_multistep: the same, its second-order steps as lp_multistep and its Euler steps (the first one, the step
+        # to sigma = 0) as lp_midpoint on x alone; the scalars also as device tensors for the un-fused update.  Its draw
+        # is multiplied by sigma_up = 0 and not taken
+        if sampler == "res_multistep":
+            rows = res_multistep_step(sched.sigmas.to(dev))
+            self.multistep = [(_native.Multistep(*v) if second else _native.Midpoint(v[0], v[1]), second)
+                              for second, *v in rows]
+            self.res_scalars = torch.tensor([v for _, *v in rows], dtype=torch.float32, device=dev)
         # dpm_2: per outer step (lp_midpoint of call A's update, of call B's or None, the index of call B's row), the
         # rows of the midpoint calls (their own tables, model times, sigmas and active counts), and the sampler's
         # scalars as device tensors for the un-fused update.  No draw of its own
@@ -463,6 +518,16 @@ class GraphedJob:
                          for i, (sigma, c_cur, c_prev1, c_prev2, order) in enumerate(rows)]
             self.d_ring = (mk(), mk(), mk())
             self.deis_scalars = torch.tensor([r[:4] for r in rows], dtype=torch.float32, device=dev)
+        # gradient_estimation: per outer step (lp_gradient_estimation, whether it reads the previous step's d, whether a
+        # later step reads its own), and a ring of two derivative buffers: step i writes d_ring[i % 2] and reads
+        # d_ring[(i - 1) % 2], so every per-step graph bakes in a fixed pair.  No draw of its own
+        self.ge = None
+        if sampler == "gradient_estimation":
+            rows = gradient_estimation_step(sched.sigmas.to(dev))
+            self.ge = [(_native.GradientEstimation(sigma, dt, gm1, int(final)), reads, keep)
+                       for sigma, dt, gm1, reads, final, keep in rows]
+            self.d_ring = (mk(), mk())
+            self.ge_scalars = torch.tensor([r[:2] for r in rows], dtype=torch.float32, device=dev)
         draws = lambda n: 0 if n <= 0 else (n if merged else 2 * n - 1)   # noqa: E731  one wrapper call's draws
         self._call_draws = draws
         self.draws_before = [0]
@@ -520,15 +585,19 @@ class GraphedJob:
         st = self.sched.steps[i]
         coef = (st.sigma_next - st.sigma) / st.sigma
         anc = self.ancestral[i] if self.ancestral is not None else None
-        ms, old, dz = None, None, None
+        ms, old, dz, ge = None, None, None, None
         if self.multistep is not None:
             ms = self.multistep[i]
             old = self.denoised_buffer(i - 1, want_out) if ms[1] else None
+        euler_mp = ms is not None and isinstance(ms[0], _native.Midpoint)   # a res_multistep Euler step
         if self.deis is not None:     # (lp_deis, d_out, d_prev1, d_prev2)
             step, order, keep = self.deis[i]
             ring = self.d_ring
             dz = (step, ring[i % 3] if keep else None, ring[(i - 1) % 3] if order >= 2 else None,
                   ring[(i - 2) % 3] if order >= 3 else None)
+        if self.ge is not None:       # (lp_gradient_estimation, d_out, d_prev)
+            step, reads, keep = self.ge[i]
+            ge = (step, self.d_ring[i % 2] if keep else None, self.d_ring[(i - 1) % 2] if reads else None)
         last = i + 1 == len(self.sched.steps)
         plan.used = self.draws_before[i]
         out = self.out if (want_out or not self.fused_euler) else None
@@ -539,13 +608,36 @@ class GraphedJob:
         eng._launch_sequence(self.x, self.y, self.noise, self.mask, self._dims, self.tables[i], self.t_model[i],
                              self.sigma[i], self.c, out, self.active[i], plan, False, self.model_options, self.seed,
                              None, self.rng_state.data_ptr(), discard_heads=heads_discardable(self.model_options),
-                             euler_coef=coef if (self.fused_euler and anc is None and ms is None and dz is None) else None,
+                             euler_coef=coef if (self.fused_euler and anc is None and ms is None and dz is None
+                                                 and ge is None) else None,
                              skip_prologue=(self.fused_euler and i > 0) or (i == 0 and self.first_replace_noop),
                              next_table=self.tables[i + 1] if (self.fused_euler and not last) else None,
                              ancestral=anc if self.fused_euler else None,
-                             multistep=(ms[0], old) if (self.fused_euler and ms is not None) else None,
-                             deis=dz if self.fused_euler else None)
+                             multistep=(ms[0], old) if (self.fused_euler and ms is not None and not euler_mp) else None,
+                             midpoint=(ms[0], self.x, self.x) if (self.fused_euler and euler_mp) else None,
+                             deis=dz if self.fused_euler else None, ge=ge if self.fused_euler else None)
         if self.fused_euler:
+            return
+        if self.sampler == "res_multistep":     # sample_res_multistep's tensor ops, in its order
+            sc = self.res_scalars[i]
+            if euler_mp:
+                self.x.copy_(self.x + ((self.x - out) / sc[0]) * sc[1])
+            else:     # sigma_fn(h) * x + h * (b1 * denoised + b2 * old_denoised), h = -em1, b2 = -c_old
+                self.x.copy_(sc[0] * self.x + (-sc[1]) * (sc[2] * out + (-sc[3]) * old))
+            return
+        if ge is not None:     # sample_gradient_estimation's tensor ops, in its order
+            step, d_out, d_prev = ge
+            sc = self.ge_scalars[i]
+            d = (self.x - out) / sc[0]
+            if step.final:
+                self.x.copy_(out)
+            else:
+                x = self.x + d * sc[1]
+                if d_prev is not None:
+                    x = x + (step.gm1 * (d - d_prev)) * sc[1]
+                self.x.copy_(x)
+            if d_out is not None:
+                d_out.copy_(d)
             return
         if dz is not None:     # sample_deis's tensor ops, in its order
             sc = self.deis_scalars[i]
@@ -769,8 +861,8 @@ class SamplerGraphJob:
     """ANY deterministic k-diffusion sampler around the per-sigma wrapper as ONE CUDA graph per job.
 
     `runner.GraphedJob` owns the sampler loop, so it only serves the samplers it restates (euler, euler_ancestral,
-    dpmpp_2m, dpm_2, deis).  For the other samplers (heun, res_multistep, ...) the loop is third-party Python that
-    calls the wrapper with sigma values only it knows.  But for a fixed schedule that sequence is deterministic: the node layer records it during the first,
+    dpmpp_2m, dpm_2, deis, res_multistep, gradient_estimation).  For the other samplers (heun, ...) the loop is
+    third-party Python that calls the wrapper with sigma values only it knows.  But for a fixed schedule that sequence is deterministic: the node layer records it during the first,
     eager job of a configuration (`KSamplerX0Inpaint.trace`), this class turns every recorded call into device
     constants (`engine.plan_item`) and then runs the sampler function ITSELF under stream capture -- its Python runs
     once, at capture -- with the wrapper serving the planned calls (`engine.run_planned`: no read-back, no copies).

@@ -142,6 +142,54 @@ def deis_step(sampler_fn, sigmas: torch.Tensor):
     return rows
 
 
+def res_multistep_step(sigmas: torch.Tensor):
+    """[(second, a, b, c, d)] for every outer step of ComfyUI's sample_res_multistep (res_multistep, eta = 0) on
+    `sigmas`: an Euler step (False, sigma_i, dt, 0, 0), x = x + ((x - denoised) / sigma_i) * dt with dt = sigma_next -
+    sigma_i, or a second-order step (True, ratio, em1, c_cur, c_old) in lp_multistep's form, x = ratio*x -
+    em1*(c_cur*denoised - c_old*old_denoised), with ratio = sigma_fn(h), em1 = -h, c_cur = b1 and c_old = -b2.
+
+    As `dpmpp_2m_step`: the sampler's own torch expressions (get_ancestral_step with eta = 0, the phi functions,
+    nan_to_num) on its own 0-d fp32 tensors where `sigmas` lives, read back once.  The sampler takes the Euler step on
+    its first step and where sigma_down = sigma_next is 0."""
+    sigma_fn = lambda t: t.neg().exp()              # noqa: E731
+    t_fn = lambda sigma: sigma.log().neg()          # noqa: E731
+    phi1_fn = lambda t: torch.expm1(t) / t          # noqa: E731
+    phi2_fn = lambda t: (phi1_fn(t) - 1.0) / t      # noqa: E731
+    host = [float(v) for v in sigmas.detach().cpu()]
+    rows = []
+    for i in range(len(host) - 1):
+        sigma_down = sigmas[i + 1]              # get_ancestral_step(sigma_i, sigma_next, eta=0)
+        if i == 0 or host[i + 1] == 0.0:
+            z = torch.zeros_like(sigma_down)
+            rows.append(torch.stack([sigmas[i], sigma_down - sigmas[i], z, z]))
+            continue
+        t, t_old, t_next, t_prev = t_fn(sigmas[i]), t_fn(sigmas[i]), t_fn(sigma_down), t_fn(sigmas[i - 1])
+        h = t_next - t
+        c2 = (t_prev - t_old) / h
+        phi1_val, phi2_val = phi1_fn(-h), phi2_fn(-h)
+        b1 = torch.nan_to_num(phi1_val - phi2_val / c2, nan=0.0)
+        b2 = torch.nan_to_num(phi2_val / c2, nan=0.0)
+        rows.append(torch.stack([sigma_fn(h), -h, b1, -b2]))
+    vals = torch.stack(rows).cpu().tolist() if rows else []
+    return [(i > 0 and host[i + 1] != 0.0, *v) for i, v in enumerate(vals)]
+
+
+def gradient_estimation_step(sigmas: torch.Tensor, ge_gamma: float = 2.0):
+    """[(sigma, dt, gm1, reads_old, final, keep)] for every outer step of ComfyUI's sample_gradient_estimation on
+    `sigmas`: d = (x - denoised) / sigma; x = denoised on the step to sigma = 0 (final), else x = x + d*dt and, when the
+    step reads the previous step's d (i >= 1), x = x + (gm1*(d - old_d))*dt.  keep: a later step reads this step's d.
+
+    sigma and dt = sigma_next - sigma are the sampler's 0-d fp32 tensors where `sigmas` lives, read back once; gm1 is
+    the fp32 value of the Python float ge_gamma - 1, which torch rounds to the tensor's type before it multiplies."""
+    host = [float(v) for v in sigmas.detach().cpu()]
+    n = len(host) - 1
+    vals = torch.stack([sigmas[:-1], sigmas[1:] - sigmas[:-1]], 1).cpu().tolist() if n > 0 else []
+    gm1 = float(torch.tensor(ge_gamma - 1, dtype=torch.float32))
+    final = [host[i + 1] == 0.0 for i in range(n)]
+    reads = [i >= 1 and not final[i] for i in range(n)]
+    return [(v[0], v[1], gm1, reads[i], final[i], i + 1 < n and reads[i + 1]) for i, v in enumerate(vals)]
+
+
 @dataclass
 class Hyper:
     step_size: float

@@ -365,8 +365,108 @@ def sample_deis(model, x, sigmas, extra_args=None, callback=None, disable=None, 
     return x_next
 
 
+def get_ancestral_step(sigma_from, sigma_to, eta=1.0):
+    """k-diffusion's get_ancestral_step: (sigma_down, sigma_up) of an ancestral step; (sigma_to, 0.) when eta is 0."""
+    if not eta:
+        return sigma_to, 0.0
+    sigma_up = min(sigma_to, eta * (sigma_to ** 2 * (sigma_from ** 2 - sigma_to ** 2) / sigma_from ** 2) ** 0.5)
+    sigma_down = (sigma_to ** 2 - sigma_up ** 2) ** 0.5
+    return sigma_down, sigma_up
+
+
+def default_noise_sampler(x, seed=None):
+    """ComfyUI's default_noise_sampler: randn of x's shape from a private generator on x's device, seeded once, when a
+    seed is given; from the global generator otherwise."""
+    if seed is not None:
+        generator = torch.Generator(device=x.device)
+        generator.manual_seed(seed)
+    else:
+        generator = None
+    return lambda sigma, sigma_next: torch.randn(x.size(), dtype=x.dtype, layout=x.layout, device=x.device,
+                                                 generator=generator)
+
+
+@torch.no_grad()
+def res_multistep(model, x, sigmas, extra_args=None, callback=None, disable=None, s_noise=1.0, noise_sampler=None,
+                  eta=1.0):
+    """ComfyUI's res_multistep without its cfg_pp branch: RES (arXiv 2308.02157), a second-order exponential multistep
+    update from this step's and the previous step's denoised latents, Euler on the first step and on the step to
+    sigma_down = 0, and an ancestral draw scaled by sigma_up.
+
+    Written from ComfyUI's comfy/k_diffusion/sampling.py as its author knows it, and not compared with ComfyUI itself,
+    which is not a dependency of this project."""
+    extra_args = {} if extra_args is None else extra_args
+    seed = extra_args.get("seed", None)
+    noise_sampler = default_noise_sampler(x, seed=seed) if noise_sampler is None else noise_sampler
+    s_in = x.new_ones([x.shape[0]])
+    sigma_fn = lambda t: t.neg().exp()              # noqa: E731
+    t_fn = lambda sigma: sigma.log().neg()          # noqa: E731
+    phi1_fn = lambda t: torch.expm1(t) / t          # noqa: E731
+    phi2_fn = lambda t: (phi1_fn(t) - 1.0) / t      # noqa: E731
+    old_sigma_down = None
+    old_denoised = None
+    for i in range(len(sigmas) - 1):
+        denoised = model(x, sigmas[i] * s_in, **extra_args)
+        sigma_down, sigma_up = get_ancestral_step(sigmas[i], sigmas[i + 1], eta=eta)
+        if callback is not None:
+            callback({"x": x, "i": i, "sigma": sigmas[i], "sigma_hat": sigmas[i], "denoised": denoised})
+        if sigma_down == 0 or old_denoised is None:
+            d = (x - denoised) / _append_dims(sigmas[i], x.ndim)
+            x = x + d * (sigma_down - sigmas[i])
+        else:
+            t, t_old, t_next, t_prev = t_fn(sigmas[i]), t_fn(old_sigma_down), t_fn(sigma_down), t_fn(sigmas[i - 1])
+            h = t_next - t
+            c2 = (t_prev - t_old) / h
+            phi1_val, phi2_val = phi1_fn(-h), phi2_fn(-h)
+            b1 = torch.nan_to_num(phi1_val - phi2_val / c2, nan=0.0)
+            b2 = torch.nan_to_num(phi2_val / c2, nan=0.0)
+            x = sigma_fn(h) * x + h * (b1 * denoised + b2 * old_denoised)
+        if sigmas[i + 1] > 0:
+            x = x + noise_sampler(sigmas[i], sigmas[i + 1]) * s_noise * sigma_up
+        old_denoised = denoised
+        old_sigma_down = sigma_down
+    return x
+
+
+@torch.no_grad()
+def sample_res_multistep(model, x, sigmas, extra_args=None, callback=None, disable=None, s_noise=1.0,
+                         noise_sampler=None):
+    """ComfyUI's sample_res_multistep: res_multistep with eta = 0 (its draw is multiplied by sigma_up = 0)."""
+    return res_multistep(model, x, sigmas, extra_args=extra_args, callback=callback, disable=disable, s_noise=s_noise,
+                         noise_sampler=noise_sampler, eta=0.0)
+
+
+@torch.no_grad()
+def sample_gradient_estimation(model, x, sigmas, extra_args=None, callback=None, disable=None, ge_gamma=2.0):
+    """ComfyUI's gradient-estimation sampler without its cfg_pp branch: an Euler step corrected, from the second step
+    on, by (ge_gamma - 1) times the change of the derivative; the step to sigma = 0 returns the denoised latent.
+
+    Written from ComfyUI's comfy/k_diffusion/sampling.py as its author knows it, and not compared with ComfyUI itself,
+    which is not a dependency of this project.  ComfyUI has also shipped an older form (x + (ge_gamma d + (1 - ge_gamma)
+    old_d) dt, no x = denoised at sigma = 0); this is the newer one."""
+    extra_args = {} if extra_args is None else extra_args
+    s_in = x.new_ones([x.shape[0]])
+    old_d = None
+    for i in range(len(sigmas) - 1):
+        denoised = model(x, sigmas[i] * s_in, **extra_args)
+        d = (x - denoised) / _append_dims(sigmas[i], x.ndim)
+        if callback is not None:
+            callback({"x": x, "i": i, "sigma": sigmas[i], "sigma_hat": sigmas[i], "denoised": denoised})
+        dt = sigmas[i + 1] - sigmas[i]
+        if sigmas[i + 1] == 0:
+            x = denoised
+        else:
+            x = x + d * dt
+            if i >= 1:
+                d_bar = (ge_gamma - 1) * (d - old_d)
+                x = x + d_bar * dt
+        old_d = d
+    return x
+
+
 _SAMPLER_FUNCTIONS = {"euler": sample_euler, "heun": sample_heun, "euler_ancestral": sample_euler_ancestral,
-                      "dpmpp_2m": sample_dpmpp_2m, "dpm_2": sample_dpm_2, "deis": sample_deis}
+                      "dpmpp_2m": sample_dpmpp_2m, "dpm_2": sample_dpm_2, "deis": sample_deis,
+                      "res_multistep": sample_res_multistep, "gradient_estimation": sample_gradient_estimation}
 # ComfyUI's KSampler takes one step more for these and drops the penultimate sigma (the samplers minicomfy has)
 DISCARD_PENULTIMATE_SIGMA_SAMPLERS = {"dpm_2"}
 
