@@ -35,8 +35,8 @@ extern "C" {
  * rejected with LP_ERR_INVALID, so no earlier caller can have set it); 2 = lp_multistep and
  * lp_boundary_multistep (a new entry point: nothing an earlier caller binds changes).  Later entry points
  * (lp_midpoint and lp_boundary_midpoint, lp_deis and lp_boundary_deis, lp_gradient_estimation and
- * lp_boundary_gradient_estimation) leave LP_ABI_MINOR at 2: a caller detects one by its symbol, which is
- * how lanpaint_b200._native binds every entry point (by name). */
+ * lp_boundary_gradient_estimation, lp_heun and lp_boundary_heun) leave LP_ABI_MINOR at 2: a caller detects one by
+ * its symbol, which is how lanpaint_b200._native binds every entry point (by name). */
 #define LP_ABI_MINOR 2
 #define LP_TABLE_STRIDE 32 /* floats per table row (one 128-byte line), layout below */
 
@@ -496,6 +496,36 @@ int lp_boundary_gradient_estimation(const lp_heads* model_out, const float* y, c
                                     const lp_known* known, float* x_inout, float* out, float* d_out,
                                     const float* d_prev, const lp_gradient_estimation* step, const float* next_table,
                                     const lp_dims* dims, lp_stream_t stream);
+
+/* The corrector of k-diffusion's sample_heun (no churn, so sigma_hat = sigma_i): x = x + ((d + d_2) / 2) * dt with
+ * d = (x - denoised) / sigma_i from the step's first wrapper call and d_2 = (x_2 - denoised_2) / sigma_next from its
+ * second, at x_2 = x + d*dt.  The host evaluates the three scalars with the sampler's own torch expressions on the
+ * schedule, on the device the sampler runs on, and reads them back.  Per outer step i with sigma_next > 0:
+ *   predictor  lp_boundary_midpoint, sigma = sigma_i, dt,   x_in = x_base = X,  x_out = X2, out = OUT
+ *   corrector  lp_boundary_heun,                             x = X, x2 = X2, out_prev = OUT
+ * and the step to sigma_next = 0 is lp_boundary_midpoint with x_in = x_base = x_out = X. */
+typedef struct lp_heun {
+  float sigma;      /* sigma_i, the sigma d divides by */
+  float sigma_next; /* sigma_{i+1}, the sigma d_2 divides by */
+  float dt;         /* sigma_{i+1} - sigma_i */
+} lp_heun;
+
+/* The boundary of the second wrapper call of an outer step of a host-owned Heun loop in ONE pass: lp_boundary_known
+ * with the Euler update replaced by sample_heun's corrector:
+ *   den = model_out->combine ? b + (a - b)*cfg : a
+ *   out = mask ? y : den                                                written when out != NULL
+ *   x   = x + ((((x - out_prev) / sigma) + ((x2 - out) / sigma_next)) / 2) * dt
+ *   x   = mask ? rep_noise*noise + rep_y*y : x  (row of next_table)     when next_table != NULL
+ * out_prev is the first call's out (its pasted denoised latent) and x2 the state the second call ran on.  d is
+ * recomputed from x and out_prev with the sampler's operations on the sampler's inputs (x is not written between the
+ * two calls), so it has the sampler's bits.  Every operation of the update is the single correctly rounded fp32
+ * operation the eager sampler issues (sub, div, add, mul by 1/2, mul, add; never contracted), so x equals the un-fused
+ * route's bit for bit.  x, x2 and out_prev are read only where the update survives (free positions; known positions
+ * too when next_table == NULL).  x, x2, out_prev and out overlap none of each other.  known may be NULL (dense y /
+ * noise / mask). */
+int lp_boundary_heun(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                     const lp_known* known, float* x, const float* x2, const float* out_prev, float* out,
+                     const lp_heun* step, const float* next_table, const lp_dims* dims, lp_stream_t stream);
 
 /* Final denoise of an outer step straight from raw cond / uncond predictions:
  *   out = mask ? y : uncond + (cond - uncond)*cfg ;  if x_inout != NULL: x = x + (x - out)*euler_coef. */

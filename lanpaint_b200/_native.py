@@ -26,7 +26,7 @@ SYMBOLS = (
     "lp_abi_version", "lp_status_string", "lp_last_cuda_error", "lp_set_option", "lp_selftest_index_math", "lp_selftest_box_muller", "lp_selftest_normal_fast", "lp_build_coef_table", "lp_build_coef_table_dt",
     "lp_torch_randn_geometry", "lp_pack_mask_f32", "lp_prologue_f32", "lp_substep", "lp_substep_f32", "lp_substep_cfg_f32", "lp_advance_f32",
     "lp_boundary", "lp_boundary_ancestral", "lp_boundary_multistep", "lp_boundary_midpoint", "lp_boundary_deis", "lp_boundary_gradient_estimation",
-    "lp_synth_denoiser", "lp_known_words", "lp_pack_known", "lp_substep_known", "lp_boundary_known",
+    "lp_boundary_heun", "lp_synth_denoiser", "lp_known_words", "lp_pack_known", "lp_substep_known", "lp_boundary_known",
     "lp_epilogue_f32", "lp_epilogue_euler_f32", "lp_step_boundary_f32", "lp_epilogue_cfg_f32", "lp_stop_stats_f32", "lp_fill_normal_f32", "lp_synth_denoiser_f32", "lp_l2_persist_capacity", "lp_l2_persist_set", "lp_l2_persist_clear", "lp_l2_flush", "lp_torch_cpu_randn_f32",
 )
 
@@ -85,6 +85,11 @@ class GradientEstimation(C.Structure):
     """lp_gradient_estimation: one step of sample_gradient_estimation, x = x + d*dt [+ (gm1*(d - d_prev))*dt], or
     x = out when final; d = (x - out)/sigma."""
     _fields_ = [("sigma", C.c_float), ("dt", C.c_float), ("gm1", C.c_float), ("final", C.c_int)]
+
+
+class Heun(C.Structure):
+    """lp_heun: the corrector of sample_heun, x = x + ((((x - out_prev)/sigma) + ((x2 - out)/sigma_next)) / 2) * dt."""
+    _fields_ = [("sigma", C.c_float), ("sigma_next", C.c_float), ("dt", C.c_float)]
 
 
 _lib: Optional[C.CDLL] = None
@@ -157,6 +162,9 @@ def load() -> C.CDLL:
     lib.lp_boundary_gradient_estimation.restype = i32
     lib.lp_boundary_gradient_estimation.argtypes = [C.POINTER(Heads), p, p, p, C.POINTER(Known), p, p, p, p,
                                                     C.POINTER(GradientEstimation), p, C.POINTER(Dims), p]
+    lib.lp_boundary_heun.restype = i32
+    lib.lp_boundary_heun.argtypes = [C.POINTER(Heads), p, p, p, C.POINTER(Known), p, p, p, p, C.POINTER(Heun), p,
+                                     C.POINTER(Dims), p]
     lib.lp_synth_denoiser.restype = i32
     lib.lp_synth_denoiser.argtypes = [p, p, p, i32, i64, p, p]
     lib.lp_substep_f32.restype = i32

@@ -398,7 +398,9 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
         res_multistep (on by default when extra_args has a seed), its second-order step inside lp_boundary_multistep
         and its Euler steps inside lp_boundary_midpoint, and gradient_estimation (on by default), its update and
         the previous step's derivative inside lp_boundary_gradient_estimation; each of the last two only when a
-        check of the sampler function on a tiny CPU problem shows the form the loop restates;
+        check of the sampler function on a tiny CPU problem shows the form the loop restates; with the option
+        "fused_heun" (and the same check) heun runs there too, both of its wrapper calls per step in the loop, its
+        predictor inside lp_boundary_midpoint and its corrector inside lp_boundary_heun;
       * any other deterministic sampler: the first job records which sigmas the sampler hands the wrapper, then
         k-diffusion's sampler function itself is captured into ONE graph (`runner.SamplerGraphJob`);
       * anything else (samplers that draw their own noise, early stop, AV packs, mask schedules): k-diffusion's own
@@ -485,6 +487,9 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             fused = dict(sampler="res_multistep")
         elif KSAMPLER._fused_gradient_estimation_ok(self, model_k, denoise_mask, model_options, engine):
             fused = dict(sampler="gradient_estimation")
+        elif opts.get("fused_heun", False) and KSAMPLER._fused_heun_ok(self, model_k, denoise_mask, model_options,
+                                                                        engine):
+            fused = dict(sampler="heun", sampler_fn=self.sampler_function)
         elif KSAMPLER._fused_euler_ok(self, model_k, denoise_mask, model_options, engine):
             fused = {}
         if opts.get("fused_sampler", True) and fused is not None:
@@ -621,6 +626,16 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             return False
         return (KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine)
                 and _restates(fn, "gradient_estimation"))
+
+    def _fused_heun_ok(self, model_k, denoise_mask, model_options, engine) -> bool:
+        """True when k-diffusion's sample_heun around the per-sigma wrapper is the host-owned loop of
+        runner.GraphedJob(sampler="heun"): the sampler without extra options (no churn), the exclusions of
+        `_fused_euler_ok`, and the form check of `_restates`, which also turns away a sample_heun that draws from the
+        global generator without churn (k-diffusion's original)."""
+        fn = self.sampler_function
+        if getattr(fn, "__name__", "") != "sample_heun" or self.extra_options:
+            return False
+        return KSAMPLER._fused_loop_ok(model_k, denoise_mask, model_options, engine) and _restates(fn, "heun")
 
     def _fused_euler(self, model_k, entry, engine, x_init, latent_image, denoise_mask, model_options, seed, flow,
                      early_stop, callback, total_steps, use_graph, opts, sampler=None):
@@ -782,14 +797,32 @@ def _gradient_estimation_form(model, x, sigmas):
     return x
 
 
-_FORMS = {"res_multistep": _res_multistep_form, "gradient_estimation": _gradient_estimation_form}
+def _heun_form(model, x, sigmas):
+    """runner.GraphedJob(sampler="heun")'s update from `heun_step`'s scalars, in x's dtype."""
+    from .schedule import heun_step
+    for i, (sigma, dt, sigma_next, corrector) in enumerate(heun_step(sigmas.to(torch.float32))):
+        d = (x - model(x, sigmas[i])) / sigma
+        if not corrector:
+            x = x + d * dt
+            continue
+        x_2 = x + d * dt
+        d_2 = (x_2 - model(x_2, sigmas[i + 1])) / sigma_next
+        x = x + (d + d_2) / 2 * dt
+    return x
+
+
+_FORMS = {"res_multistep": _res_multistep_form, "gradient_estimation": _gradient_estimation_form,
+          "heun": _heun_form}
 _FORM_OK = {}     # (sampler function, sampler) -> whether the function computes the form of that fused loop
 
 
 def _restates(fn, sampler: str) -> bool:
     """Whether the sampler function `fn` computes what the fused loop of `sampler` restates: `fn` runs once, in fp64
     on the CPU, around an affine stand-in network, on a 5-step schedule that ends at 0 and on a window that ends above
-    it, and its results must match the loop's update from its own fp32 scalars to 1e-5.  Cached per function."""
+    it, and its results must match the loop's update from its own fp32 scalars to 1e-5.  The function must also leave
+    the global generator where it found it: the fused loops take no draw from it (k-diffusion's original sample_heun
+    draws a randn_like every step even without churn, which on the device would shift every later Langevin draw).  The
+    generator's state is put back afterwards, so the check consumes nothing.  Cached per function."""
     key = (fn, sampler)
     ok = _FORM_OK.get(key)
     if ok is None:
@@ -798,17 +831,22 @@ def _restates(fn, sampler: str) -> bool:
         bias = torch.randn(2, 3, 4, 4, generator=g, dtype=torch.float64)
         model = lambda x, sigma, **kw: 0.75 * x + 0.25 * bias   # noqa: E731
         ok = True
-        for sig in ([5.0, 2.5, 1.1, 0.4, 0.1, 0.0], [5.0, 2.5, 1.1, 0.4]):
-            sigmas = torch.tensor(sig, dtype=torch.float64)
-            try:
-                got = fn(model, x0.clone(), sigmas, extra_args={"seed": 0}, callback=None, disable=True)
-            except Exception:
-                ok = False
-                break
-            want = _FORMS[sampler](model, x0.clone(), sigmas)
-            if not float((got - want).abs().max()) <= 1e-5 * float(want.abs().max()):
-                ok = False
-                break
+        state = torch.default_generator.get_state()
+        try:
+            for sig in ([5.0, 2.5, 1.1, 0.4, 0.1, 0.0], [5.0, 2.5, 1.1, 0.4]):
+                sigmas = torch.tensor(sig, dtype=torch.float64)
+                try:
+                    got = fn(model, x0.clone(), sigmas, extra_args={"seed": 0}, callback=None, disable=True)
+                except Exception:
+                    ok = False
+                    break
+                want = _FORMS[sampler](model, x0.clone(), sigmas)
+                if not float((got - want).abs().max()) <= 1e-5 * float(want.abs().max()):
+                    ok = False
+                    break
+            ok = ok and torch.equal(torch.default_generator.get_state(), state)
+        finally:
+            torch.default_generator.set_state(state)
         _FORM_OK[key] = ok
     return ok
 

@@ -11,6 +11,8 @@
 //   boundary_deis_kernel
 //                       the same boundary for ComfyUI's sample_deis (DEIS, third order), writing the step's derivative
 //   boundary_ge_kernel  the same boundary for ComfyUI's sample_gradient_estimation, writing the step's derivative
+//   boundary_heun_kernel
+//                       the same boundary for the second wrapper call of k-diffusion's sample_heun (its corrector)
 //   advance_kernel      one un-fused advance_time_overdamped             lanpaint.py:232-254
 //   stop_stats_kernel   early-stop masked reductions                     earlystop.py:32-55,238-313
 #include "lp_common.cuh"
@@ -1428,6 +1430,160 @@ static int boundary_ge_impl(const lp_heads* mo, const float* y, const float* noi
   }
 }
 
+// ---- the boundary of the second wrapper call of a host-owned Heun loop ------------------------------------------
+// k-diffusion's sample_heun issues, after its second wrapper call, sub, div (d_2), add, div by 2, mul, add as eager
+// kernels, with d from its first call and per-step 0-d tensors the host hands in as lp_heun; lp_boundary_heun does
+// them in the boundary's one pass, each as the same correctly rounded fp32 operation, and recomputes d from x and the
+// first call's denoised latent with the sampler's sub, div.
+struct HeunArgs {
+  BoundaryArgs b;       // b.x is x, read and written; coef is unused
+  lp_heun st;
+  const float* x2;      // the state the second call ran on
+  const float* prev;    // the first call's out
+};
+
+// per element: den = combine ? b + (a-b) cfg : a ; o = known ? y : den ; d = (x - prev) / sigma ;
+// d2 = (x2 - o) / sigma_next ; x = x + ((d + d2) * 0.5) dt ; x = known ? rn n + ry y : x
+__device__ __forceinline__ void heun_element(float a, float b, float y, float nz, float v2, float pv, bool known,
+                                             float& x, float& o, bool combine, float cfg, const lp_heun& st, bool next,
+                                             float rn, float ry) {
+  const float den = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
+  o = known ? y : den;
+  const float d = __fdiv_rn(__fsub_rn(x, pv), st.sigma);
+  const float d2 = __fdiv_rn(__fsub_rn(v2, o), st.sigma_next);
+  // torch divides by the Python scalar 2 as a multiply by 0.5: the same bits, there being no flush to zero
+  const float u = __fadd_rn(x, __fmul_rn(__fmul_rn(__fadd_rn(d, d2), 0.5f), st.dt));
+  x = next && known ? fmaf(rn, nz, ry * y) : u;  // the replace step rounds as prologue_kernel does
+}
+
+// boundary_kernel's form and operand skipping; x, x2 and the first call's out are read where x's update survives
+template <int N, typename H, bool kPk>
+__global__ void __launch_bounds__(kBlock) boundary_heun_kernel(const HeunArgs q) {
+  pdl_prologue();
+  const BoundaryArgs& p = q.b;
+  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= p.g.total) return;
+  const uint64_t dead = l2_policy_dead(p.l2);
+  uint32_t row, mi;
+  locate(p.g, i, row, mi);
+  const bool next = p.next_table != nullptr;
+  float av[N], bv[N], yv[N], xv[N], nv[N], v2[N], pv[N], ov[N];
+  bool known[N];
+  uint32_t kb = 0, kidx = 0;
+  if constexpr (kPk) {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
+    if constexpr (N == 4) {
+      known_quad(w, i, kb, kidx);
+    } else {
+      kb = (w.x >> (i & 31u)) & 1u;
+      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
+    }
+#pragma unroll
+    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
+  } else {
+    load_m<N>(p.mask, mi, known);
+  }
+  bool any_known = false, any_free = false;
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    any_known |= known[j];
+    any_free |= !known[j];
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = v2[j] = pv[j] = 0.f;
+  if constexpr (kPk) {
+    if constexpr (N == 4) {
+      gather_known4<false>(p.yk, kb, kidx, yv);
+    } else {
+      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
+    }
+  } else {
+    load_f_ro<N>(p.y, i, yv);
+  }
+  if (any_free) {
+    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
+    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
+  }
+  if (any_free || !next) {  // somewhere in the vector x's update is not overwritten by the replace step
+    load_f<N>(p.x, i, xv);
+    load_head_ro<N, float>(q.x2, i, v2, dead);    // the next predictor overwrites it unread
+    load_head_ro<N, float>(q.prev, i, pv, dead);  // so does the next first call
+  }
+  float rn = 0.f, ry = 0.f;
+  if (next) {
+    if constexpr (kPk) {
+      if constexpr (N == 4) {
+        gather_known4<false>(p.nk, kb, kidx, nv);
+      } else {
+        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
+      }
+    } else {
+      if (any_known) load_f_ro<N>(p.noise, i, nv);
+    }
+    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
+    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j)
+    heun_element(av[j], bv[j], yv[j], nv[j], v2[j], pv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st, next,
+                 rn, ry);
+  if (p.out) store_f<N>(p.out, i, ov, dead);
+  store_f<N>(p.x, i, xv);  // normal policy: the next network call reads x first
+  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
+    if (p.discard) {
+      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
+      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
+        __syncwarp();           // every lane's head loads are used
+        discard_line<H>(p.a, i, end);
+        if (p.b) discard_line<H>(p.b, i, end);
+      }
+    }
+  }
+}
+
+template <typename H>
+int heun_dispatch(const HeunArgs& q, bool v4, cudaStream_t s) {
+  const uint32_t total = q.b.g.total;
+  if (q.b.kwords) {
+    if (v4) launch_kernel(boundary_heun_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_heun_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
+  } else {
+    if (v4) launch_kernel(boundary_heun_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
+    else launch_kernel(boundary_heun_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
+  }
+  return check_launch();
+}
+
+static int boundary_heun_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
+                              const lp_known* known, float* x, const float* x2, const float* out_prev, float* out,
+                              const lp_heun* step, const float* next_table, const lp_dims* dims, lp_stream_t stream) {
+  if (int rc = boundary_check(mo, y, noise, mask, known, x, out, next_table)) return rc;
+  if (!step || !x || !x2 || !out_prev) return LP_ERR_INVALID;
+  HeunArgs q;
+  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  // the launch writes x and out while it reads x2 and out_prev: the four share no byte
+  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
+  const auto any = [&](const void* u, const void* v) { return u && v && (u == v || overlaps(u, v, bytes)); };
+  const void* bufs[4] = {x, x2, out_prev, out};
+  for (int k = 0; k < 4; ++k)
+    for (int l = 0; l < k; ++l)
+      if (any(bufs[k], bufs[l])) return LP_ERR_INVALID;
+  if (q.b.g.total == 0) return LP_OK;
+  boundary_args(q.b, mo, y, noise, mask, known, x, out, 0.f, next_table);
+  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x, x2, out_prev, out});  // a dropped line holds no state
+  q.st = *step;
+  q.x2 = x2;
+  q.prev = out_prev;
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
+  const bool v4 = boundary_vec4(q.b, dtype) && aligned16(x2) && aligned16(out_prev);
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (dtype) {
+    case LP_DTYPE_F32: return heun_dispatch<float>(q, v4, s);
+    case LP_DTYPE_BF16: return heun_dispatch<__nv_bfloat16>(q, v4, s);
+    default: return heun_dispatch<__half>(q, v4, s);
+  }
+}
+
 // ---- un-fused OU advance (advance_time_overdamped, lanpaint.py:232-254) --------
 struct AdvanceArgs {
   float* x;
@@ -1631,6 +1787,12 @@ extern "C" int lp_boundary_gradient_estimation(const lp_heads* model_out, const 
                                                const float* next_table, const lp_dims* dims, lp_stream_t stream) {
   return boundary_ge_impl(model_out, y, noise, mask, known, x_inout, out, d_out, d_prev, step, next_table, dims,
                           stream);
+}
+
+extern "C" int lp_boundary_heun(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                                const lp_known* known, float* x, const float* x2, const float* out_prev, float* out,
+                                const lp_heun* step, const float* next_table, const lp_dims* dims, lp_stream_t stream) {
+  return boundary_heun_impl(model_out, y, noise, mask, known, x, x2, out_prev, out, step, next_table, dims, stream);
 }
 
 extern "C" int lp_epilogue_f32(const float* model_out, const float* y, const uint8_t* mask, float* out,

@@ -534,7 +534,7 @@ class LanPaint:
     def _launch_sequence(self, xm, y, nz, pm, dims, tab, t_model, sigma_dev, cbuf, out, active, plan, call_scaling,
                          model_options, seed, stopper, rng_state, euler_coef=None, skip_prologue=False,
                          next_table=None, current_times=None, ancestral=None, discard_heads=False, multistep=None,
-                         midpoint=None, deis=None, ge=None):
+                         midpoint=None, deis=None, ge=None, heun=None):
         """discard_heads: the caller owns the network's outputs and nothing reads them once the update kernel that
         consumes them has run (`heads_discardable`), so that kernel may drop them from the L2 unwritten
         (LP_HEADS_DEAD).  Only the fused loop's launches take it; the early-stop loop hands the heads to the stopper.
@@ -545,7 +545,10 @@ class LanPaint:
         deis: (lp_deis, d_out, d_prev1, d_prev2), each buffer or None: the boundary is lp_boundary_deis, the update of a
         host-owned sample_deis loop.
         ge: (lp_gradient_estimation, d_out, d_prev), each buffer or None: the boundary is
-        lp_boundary_gradient_estimation, the update of a host-owned sample_gradient_estimation loop."""
+        lp_boundary_gradient_estimation, the update of a host-owned sample_gradient_estimation loop.
+        heun: (lp_heun, x_base, out_prev): the boundary is lp_boundary_heun, the corrector of a host-owned sample_heun
+        loop, with x_base (the state the step started from, updated in place) as its x, xm -- the state this call's
+        sub-steps ran on -- as its x2, and out_prev the step's first call's denoised latent."""
         lib = _native.load()
         dev = xm.device
         stream = _P(_stream_ptr(dev))
@@ -708,6 +711,16 @@ class LanPaint:
                 _P(_ptr(out)), _P(_ptr(d_out)), _P(_ptr(d_prev)), C.byref(step),
                 _P(next_table.data_ptr()) if next_table is not None else None, C.byref(dims), stream)
             _native.check(rc, "lp_boundary_gradient_estimation")
+            self.launches += 1
+            return done
+        if heun is not None:
+            step, x_base, out_prev = heun
+            rc = lib.lp_boundary_heun(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
+                                      C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
+                                      _P(x_base.data_ptr()), _P(xm.data_ptr()), _P(out_prev.data_ptr()), _P(_ptr(out)),
+                                      C.byref(step), _P(next_table.data_ptr()) if next_table is not None else None,
+                                      C.byref(dims), stream)
+            _native.check(rc, "lp_boundary_heun")
             self.launches += 1
             return done
         fused_next = next_table is not None and euler_coef is not None

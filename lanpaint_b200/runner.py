@@ -21,7 +21,7 @@ import torch
 
 from . import _native
 from .schedule import (ancestral_step, deis_step, dpm_2_step, dpmpp_2m_step, effective_inner_steps,
-                       gradient_estimation_step, res_multistep_step, times_from_sigma)
+                       gradient_estimation_step, heun_step, res_multistep_step, times_from_sigma)
 
 
 class VESampling:
@@ -245,6 +245,29 @@ def dpm_2_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask,
     return x
 
 
+def heun_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask, sched: HostSchedule) -> torch.Tensor:
+    """`euler_inpaint` with k-diffusion's sample_heun (no churn) as the sampler: the un-fused definition of
+    GraphedJob(sampler="heun"), eager torch ops around both wrapper calls of a step with the sampler's own scalars
+    (`heun_step` on the schedule, on the latent's device); the second call's row is `HostSchedule.call_at`."""
+    dev = latent_image.device
+    sampling = engine.inner_model.inner_model.model_sampling
+    sig = sched.sigmas.to(dev)
+    x = sampling.noise_scaling(sig[0], noise, latent_image)
+    t = lambda v: torch.tensor(v, dtype=torch.float32, device=dev)   # noqa: E731
+    for st, (sigma_hat, dt, sigma_next, corrector) in zip(sched.steps, heun_step(sig)):
+        denoised = engine(x, latent_image, noise, st.sigma_t, mask, st.times, None, 0, n_steps=st.n_inner)
+        d = (x - denoised) / t(sigma_hat)
+        if not corrector:
+            x = x + d * t(dt)
+            continue
+        x_2 = x + d * t(dt)
+        ms = sched.call_at(sigma_next, st.sigma_next)
+        denoised_2 = engine(x_2, latent_image, noise, ms.sigma_t, mask, ms.times, None, 0, n_steps=ms.n_inner)
+        d_2 = (x_2 - denoised_2) / t(sigma_next)
+        x = x + (d + d_2) / 2 * t(dt)
+    return x
+
+
 def deis_inpaint(engine, latent_image: torch.Tensor, noise: torch.Tensor, mask, sched: HostSchedule,
                  sampler_fn) -> torch.Tensor:
     """`euler_inpaint` with ComfyUI's sample_deis (max_order 3, 'tab') as the sampler: the un-fused definition of
@@ -400,9 +423,12 @@ class GraphedJob:
     per-sigma wrapper (asserted bit-for-bit by the tests); sampler="euler_ancestral", "dpmpp_2m", "dpm_2" and "deis" are
     `euler_ancestral_inpaint`, `dpmpp_2m_inpaint`, `dpm_2_inpaint` and `deis_inpaint`.  dpm_2 makes two wrapper calls
     per outer step: call A at sigma_i on x, call B at the midpoint sigma on a second state buffer x2; both are in the
-    step's graph.  deis takes its coefficients from the sampler function `sampler_fn` (ComfyUI's sample_deis or a
-    stand-in with a `deis` module beside it).  sampler="res_multistep" (eta = 0) and "gradient_estimation" (ge_gamma =
-    2) are `res_multistep_inpaint` and `gradient_estimation_inpaint`."""
+    step's graph.  sampler="heun" (with `sampler_fn`, the sample_heun the loop stands in for) is `heun_inpaint` and has
+    the same two calls, call B at sigma_next; its corrector (lp_boundary_heun) also reads call A's denoised latent, which
+    call A therefore always writes.  deis takes its
+    coefficients from the sampler function `sampler_fn` (ComfyUI's sample_deis or a stand-in with a `deis` module
+    beside it).  sampler="res_multistep" (eta = 0) and "gradient_estimation" (ge_gamma = 2) are `res_multistep_inpaint`
+    and `gradient_estimation_inpaint`."""
 
     def __init__(self, engine, sched: HostSchedule, shape, device, flow: bool = False, fused_euler: bool = True,
                  l2_persist: bool = False, model_options=None, seed=0, external_init: bool = False,
@@ -410,13 +436,18 @@ class GraphedJob:
                  sampler_fn=None):
         import numpy as np
         from .engine import _DrawPlan
-        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m", "dpm_2", "deis", "res_multistep",
+        if sampler not in ("euler", "euler_ancestral", "dpmpp_2m", "dpm_2", "heun", "deis", "res_multistep",
                            "gradient_estimation"):
-            raise ValueError("GraphedJob owns the loops of 'euler', 'euler_ancestral', 'dpmpp_2m', 'dpm_2', 'deis', "
-                             f"'res_multistep' and 'gradient_estimation', not {sampler!r}")
+            raise ValueError("GraphedJob owns the loops of 'euler', 'euler_ancestral', 'dpmpp_2m', 'dpm_2', 'heun', "
+                             f"'deis', 'res_multistep' and 'gradient_estimation', not {sampler!r}")
         if sampler == "deis" and sampler_fn is None:
             raise ValueError("GraphedJob(sampler='deis') needs the sampler function (sampler_fn): the coefficients are "
                              "its module's")
+        if sampler == "heun" and getattr(sampler_fn, "__name__", "") != "sample_heun":
+            # the loop restates one sampler function, sample_heun without churn and without draws of its own; the caller
+            # names the function it checked (the node gate's `_restates`), and another one -- heunpp2, say -- is refused
+            raise ValueError("GraphedJob(sampler='heun') needs the sample_heun it restates (sampler_fn), run without "
+                             "churn and checked to draw nothing of its own")
         self.sampler = sampler
         self.fused_euler = fused_euler   # the sampler's update inside the step-boundary kernel instead of torch kernels
         # optional persisting-L2 window over the clean latent (re-read by every launch).  Off by default: the
@@ -437,8 +468,8 @@ class GraphedJob:
         self.x, self.y, self.noise, self.c, self.out = mk(), mk(), mk(), mk(), mk()
         # dpmpp_2m writes every step's denoised latent and reads it back at the next step: two buffers taken in turn
         self.out_pair = (self.out, mk()) if sampler in ("dpmpp_2m", "res_multistep") else None
-        # dpm_2: the midpoint call's state (x_2 of the sampler)
-        self.x2 = mk() if sampler == "dpm_2" else None
+        # dpm_2 and heun: the state of the step's second call (x_2 of the sampler)
+        self.x2 = mk() if sampler in ("dpm_2", "heun") else None
         self.mask = None
         hyper = Hyper(engine.step_size, engine.chara_lamb, engine.chara_beta, engine.min_step_frac, flow)
 
@@ -485,29 +516,37 @@ class GraphedJob:
             self.multistep = [(_native.Multistep(*v) if second else _native.Midpoint(v[0], v[1]), second)
                               for second, *v in rows]
             self.res_scalars = torch.tensor([v for _, *v in rows], dtype=torch.float32, device=dev)
-        # dpm_2: per outer step (lp_midpoint of call A's update, of call B's or None, the index of call B's row), the
-        # rows of the midpoint calls (their own tables, model times, sigmas and active counts), and the sampler's
-        # scalars as device tensors for the un-fused update.  No draw of its own
+        # dpm_2 and heun: per outer step (lp_midpoint of call A's update, call B's update -- lp_midpoint for dpm_2,
+        # lp_heun for heun -- or None, the index of call B's row), the rows of the second calls (their own tables, model
+        # times, sigmas and active counts), and the sampler's scalars (call A's sigma and dt, call B's) as device tensors
+        # for the un-fused update.  No draw of their own
         self.midpoint = None
         self.substeps = sched.substeps
-        if sampler == "dpm_2":
-            self.midpoint, mrows = [], []
-            for i, (st, (s_mid, dt_1, dt_2, mid)) in enumerate(zip(sched.steps, dpm_2_step(sched.sigmas.to(dev)))):
-                if not mid:
-                    self.midpoint.append((_native.Midpoint(st.sigma, dt_2), None, None))
+        if sampler in ("dpm_2", "heun"):
+            sig_dev = sched.sigmas.to(dev)
+            if sampler == "dpm_2":
+                calls = [(_native.Midpoint(st.sigma, dt_1 if mid else dt_2), s_mid if mid else None,
+                          _native.Midpoint(s_mid, dt_2), (s_mid, dt_2))
+                         for st, (s_mid, dt_1, dt_2, mid) in zip(sched.steps, dpm_2_step(sig_dev))]
+            else:      # call B at sigma_next, the next outer step's row whenever there is one
+                calls = [(_native.Midpoint(s, dt), s_next if corr else None, _native.Heun(s, s_next, dt), (s_next, dt))
+                         for s, dt, s_next, corr in heun_step(sig_dev)]
+            self.midpoint, mrows, scalars = [], [], []
+            for st, (pred, s_b, corr, sc_b) in zip(sched.steps, calls):
+                scalars.append([pred.sigma, pred.dt] + (list(sc_b) if s_b is not None else [0.0, 0.0]))
+                if s_b is None:
+                    self.midpoint.append((pred, None, None))
                     continue
-                ms = sched.call_at(s_mid, st.sigma_next)
+                ms = sched.call_at(s_b, st.sigma_next)
                 self.substeps += ms.n_inner
-                self.midpoint.append((_native.Midpoint(st.sigma, dt_1), _native.Midpoint(s_mid, dt_2), len(mrows)))
+                self.midpoint.append((pred, corr, len(mrows)))
                 mrows.append(call_row(ms))
             col = lambda j: (torch.from_numpy(np.stack([r[j] for r in mrows]).astype(np.float32)).to(dev)  # noqa: E731
                              if mrows else None)
             self.mid_tables, self.mid_t_model, self.mid_sigma = col(0), col(1), col(2)
             self.mid_active = [r[3] for r in mrows]
-            self.dpm_2_scalars = torch.tensor([[st.sigma, a.dt, b.sigma if b else 0.0, b.dt if b else 0.0]
-                                               for st, (a, b, _) in zip(sched.steps, self.midpoint)],
-                                              dtype=torch.float32, device=dev)
-            self.out_mid = mk() if not fused_euler else None   # the midpoint call's denoised latent (un-fused update)
+            self.call_scalars = torch.tensor(scalars, dtype=torch.float32, device=dev)
+            self.out_mid = mk() if not fused_euler else None   # call B's denoised latent (un-fused update)
         # deis: per outer step (lp_deis, order, whether a later step reads its derivative), the coefficients read back
         # once here, and a ring of three derivative buffers: step i writes d_ring[i % 3] and reads the two before it,
         # so every per-step graph bakes in a fixed triple.  No draw of its own
@@ -580,7 +619,7 @@ class GraphedJob:
 
     def _step(self, i, plan, want_out):
         if self.midpoint is not None:
-            return self._dpm_2_step(i, plan, want_out)
+            return self._two_call_step(i, plan, want_out)
         eng = self.engine
         st = self.sched.steps[i]
         coef = (st.sigma_next - st.sigma) / st.sigma
@@ -671,19 +710,22 @@ class GraphedJob:
             _native.check(rc, "lp_fill_normal_f32")
             self.x.add_(xi * step.s_noise * step.sigma_up)
 
-    def _dpm_2_step(self, i, plan, want_out):
-        """Outer step i of sample_dpm_2: call A at sigma_i on x, then (sigma_next > 0) call B at sigma_mid on x2.
-        Fused, call A's boundary is the predictor (x -> x2) with call B's replace step (its row) folded in, and call
-        B's boundary is the corrector (x2, x -> x) with the next outer step's replace step; the step to sigma = 0 is
-        one Euler boundary on x."""
+    def _two_call_step(self, i, plan, want_out):
+        """Outer step i of sample_dpm_2 or sample_heun: call A at sigma_i on x, then (sigma_next > 0) call B on x2 --
+        at sigma_mid for dpm_2, at sigma_next for heun.  Fused, call A's boundary is the predictor (x -> x2) with call
+        B's replace step (its row) folded in, and call B's boundary is the corrector (x2, x -> x; heun's also reads call
+        A's denoised latent) with the next outer step's replace step; the step to sigma = 0 is one Euler boundary on
+        x."""
         from .engine import heads_discardable
         eng = self.engine
         pred, corr, k = self.midpoint[i]
+        heun = self.sampler == "heun"
         last = i + 1 == len(self.sched.steps)
         fused = self.fused_euler
         after = self.tables[i + 1] if not last else None     # the next outer step's replace step
         plan.used = self.draws_before[i]
-        out = self.out if (want_out or not fused) else None
+        # heun's corrector reads call A's denoised latent, so call A writes it whenever there is a call B
+        out = self.out if (want_out or not fused or (heun and k is not None)) else None
         if want_out == "each":
             out = self.outs[i]
         dead = heads_discardable(self.model_options)
@@ -695,8 +737,8 @@ class GraphedJob:
                              skip_prologue=(fused and i > 0) or (i == 0 and self.first_replace_noop),
                              next_table=(self.mid_tables[k] if k is not None else after) if fused else None,
                              midpoint=(pred, self.x, x_a) if fused else None)
-        sc = self.dpm_2_scalars[i]
-        if not fused:   # sample_dpm_2's tensor ops, in its order
+        sc = self.call_scalars[i]
+        if not fused:   # the sampler's tensor ops, in its order
             d = (self.x - out) / sc[0]
             if k is None:
                 self.x.add_(d * sc[1])
@@ -705,12 +747,18 @@ class GraphedJob:
         if k is None:
             return
         plan.used = self.draws_before[i] + self._call_draws(self.active[i])
+        update = dict(heun=(corr, self.x, out)) if heun else dict(midpoint=(corr, self.x, self.x))
         eng._launch_sequence(self.x2, *common, self.mid_tables[k], self.mid_t_model[k], self.mid_sigma[k], self.c,
                              None if fused else self.out_mid, self.mid_active[k], plan, False, self.model_options,
                              self.seed, None, self.rng_state.data_ptr(), discard_heads=dead, skip_prologue=fused,
-                             next_table=after if fused else None, midpoint=(corr, self.x, self.x) if fused else None)
-        if not fused:
-            self.x.add_(((self.x2 - self.out_mid) / sc[2]) * sc[3])
+                             next_table=after if fused else None, **(update if fused else {}))
+        if fused:
+            return
+        d_2 = (self.x2 - self.out_mid) / sc[2]
+        if heun:
+            self.x.copy_(self.x + (d + d_2) / 2 * sc[3])
+        else:
+            self.x.add_(d_2 * sc[3])
 
     def _body(self, plan, want_out):
         if not self.external_init:
@@ -861,7 +909,8 @@ class SamplerGraphJob:
     """ANY deterministic k-diffusion sampler around the per-sigma wrapper as ONE CUDA graph per job.
 
     `runner.GraphedJob` owns the sampler loop, so it only serves the samplers it restates (euler, euler_ancestral,
-    dpmpp_2m, dpm_2, deis, res_multistep, gradient_estimation).  For the other samplers (heun, ...) the loop is
+    dpmpp_2m, dpm_2, heun, deis, res_multistep, gradient_estimation).  For the other samplers (heunpp2, ..., and heun
+    unless the node's option "fused_heun" routes it to the fused loop) the loop is
     third-party Python that calls the wrapper with sigma values only it knows.  But for a fixed schedule that sequence is deterministic: the node layer records it during the first,
     eager job of a configuration (`KSamplerX0Inpaint.trace`), this class turns every recorded call into device
     constants (`engine.plan_item`) and then runs the sampler function ITSELF under stream capture -- its Python runs

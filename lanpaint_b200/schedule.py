@@ -119,6 +119,21 @@ def dpm_2_step(sigmas: torch.Tensor):
     return [(v[0], v[1], v[2], host[i + 1] != 0.0) for i, v in enumerate(vals)]
 
 
+def heun_step(sigmas: torch.Tensor):
+    """[(sigma_hat, dt, sigma_next, corrector)] for every outer step of k-diffusion's sample_heun (no churn) on `sigmas`.
+
+    As `dpm_2_step`: the sampler's own torch expressions on its own 0-d fp32 tensors where `sigmas` lives, read back
+    once.  sigma_hat = sigma_i * (0 + 1) (= sigma_i), dt = sigma_next - sigma_hat.  A step makes its corrector call at
+    sigma_next when sigma_next != 0; the step to sigma = 0 is one Euler update with the same dt."""
+    host = [float(v) for v in sigmas.detach().cpu()]
+    rows = []
+    for i in range(len(host) - 1):
+        sigma_hat = sigmas[i] * (0.0 + 1)
+        rows.append(torch.stack([sigma_hat, sigmas[i + 1] - sigma_hat, sigmas[i + 1]]))
+    vals = torch.stack(rows).to(torch.float32).cpu().tolist() if rows else []
+    return [(v[0], v[1], v[2], host[i + 1] != 0.0) for i, v in enumerate(vals)]
+
+
 def deis_step(sampler_fn, sigmas: torch.Tensor):
     """[(sigma, c_cur, c_prev1, c_prev2, order)] for every outer step of ComfyUI's sample_deis (max_order = 3,
     deis_mode = 'tab') on `sigmas`: x = x + c_cur d [+ c_prev1 d_{i-1} [+ c_prev2 d_{i-2}]], d = (x - denoised) / sigma.
