@@ -66,7 +66,8 @@ struct BoundaryArgs {
   Geometry g;
 };
 
-// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; x += (x - o) coef ; x = known ? rn n + ry y : x
+// per element of boundary_tma_kernel: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; x += (x - o) coef ;
+// x = known ? rn n + ry y : x
 __device__ __forceinline__ void boundary_element(float a, float b, float y, float nz, bool known, float& x, float& o,
                                                  bool combine, float cfg, float coef, bool euler, bool next, float rn,
                                                  float ry) {
@@ -76,19 +77,26 @@ __device__ __forceinline__ void boundary_element(float a, float b, float y, floa
   if (next) x = known ? fmaf(rn, nz, ry * y) : x;
 }
 
-// kPk: the known bits and the packed y / noise of lp_known replace the uint8 mask and the dense y / noise, so y and
-// noise cost 4 B per KNOWN element each instead of 4 B per element (a 4-wide vector is rarely all-free, so the dense
-// form reads nearly all of y on a scattered mask).
-template <int N, typename H, bool kPk>
-__global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) {
-  pdl_prologue();
-  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
-  if (i >= p.g.total) return;
+// ---- the LDG boundary: one vector body, one update policy per sampler -------------------------------------------
+// boundary_vector does for the N-wide vector at element i what every LDG boundary kernel shares: the known bits, y,
+// the heads and the CFG combine, the pasted denoised value o = known ? y : d, the next replace step, the `out` store
+// and the heads' discard.  kPk: the known bits and the packed y / noise of lp_known replace the uint8 mask and the
+// dense y / noise, so y and noise cost 4 B per KNOWN element each instead of 4 B per element (a 4-wide vector is
+// rarely all-free, so the dense form reads nearly all of y on a scattered mask).  The sampler's policy U supplies
+//   u.load(i, update, dead)  its own operands; update: somewhere in the vector the new x is not overwritten by the
+//                            replace step (any_free || !next); dead: the L2 policy of operands read for the last time
+//   u.update(j, o)           element j's update from o, each operation the sampler's correctly rounded fp32 one;
+//                            returns element j's new x, which the replace step then overwrites at known positions
+//   u.store(i)               d_out where it has one, then x (after `out`)
+//   U::kDiscard              whether the launch drops the heads' lines once read: only where a warp's vectors are
+//                            one contiguous span
+template <int N, typename H, bool kPk, typename U>
+__device__ __forceinline__ void boundary_vector(const BoundaryArgs& p, uint32_t i, U& u) {
   const uint64_t dead = l2_policy_dead(p.l2);
   uint32_t row, mi;
   locate(p.g, i, row, mi);
-  const bool euler = p.x != nullptr, next = p.next_table != nullptr;
-  float av[N], bv[N], yv[N], xv[N], nv[N], ov[N];
+  const bool next = p.next_table != nullptr;
+  float av[N], bv[N], yv[N], nv[N], ov[N];
   bool known[N];
   uint32_t kb = 0, kidx = 0;
   if constexpr (kPk) {
@@ -110,8 +118,9 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
     any_known |= known[j];
     any_free |= !known[j];
   }
+  const bool update = any_free || !next;
 #pragma unroll
-  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = 0.f;
+  for (int j = 0; j < N; ++j) av[j] = bv[j] = nv[j] = 0.f;
   if constexpr (kPk) {
     if constexpr (N == 4) {
       gather_known4<false>(p.yk, kb, kidx, yv);
@@ -126,7 +135,7 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
     load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
     if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
   }
-  if (euler && (any_free || !next)) load_f<N>(p.x, i, xv);
+  u.load(i, update, dead);
   float rn = 0.f, ry = 0.f;
   if (next) {
     if constexpr (kPk) {
@@ -142,12 +151,16 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
     ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
   }
 #pragma unroll
-  for (int j = 0; j < N; ++j)
-    boundary_element(av[j], bv[j], yv[j], nv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, p.coef, euler, next, rn,
-                     ry);
+  for (int j = 0; j < N; ++j) {
+    const float d = p.combine ? __fadd_rn(bv[j], __fmul_rn(__fsub_rn(av[j], bv[j]), p.cfg)) : av[j];
+    const bool k = known[j];
+    ov[j] = k ? yv[j] : d;
+    float& x = u.update(j, ov[j]);
+    if (next) x = k ? fmaf(rn, nv[j], ry * yv[j]) : x;  // rounds as prologue_kernel does
+  }
   if (p.out) store_f<N>(p.out, i, ov, dead);
-  if (euler) store_f<N>(p.x, i, xv);
-  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
+  u.store(i);
+  if constexpr (U::kDiscard && 32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
     if (p.discard) {
       const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
       if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
@@ -157,6 +170,34 @@ __global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) 
       }
     }
   }
+}
+
+// boundary_kernel: x += (x - o) coef, where there is an x (NULL: the paste alone)
+template <int N>
+struct EulerUpdate {
+  static constexpr bool kDiscard = true;
+  float* x;
+  float coef;
+  float xv[N] = {};
+  __device__ __forceinline__ void load(uint32_t i, bool update, uint64_t) {
+    if (x && update) load_f<N>(x, i, xv);
+  }
+  __device__ __forceinline__ float& update(int j, float o) {
+    if (x) xv[j] = fmaf(xv[j] - o, coef, xv[j]);
+    return xv[j];
+  }
+  __device__ __forceinline__ void store(uint32_t i) {
+    if (x) store_f<N>(x, i, xv);
+  }
+};
+
+template <int N, typename H, bool kPk>
+__global__ void __launch_bounds__(kBlock) boundary_kernel(const BoundaryArgs p) {
+  pdl_prologue();
+  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= p.g.total) return;
+  EulerUpdate<N> u{p.x, p.coef};
+  boundary_vector<N, H, kPk>(p, i, u);
 }
 
 // TMA-staged persistent variant for HBM-bound sizes (fused Euler loop: x is always updated).  Same tile walk and
@@ -275,8 +316,30 @@ int launch_boundary_tma(const BoundaryArgs& p, cudaStream_t s) {
   return check_launch();
 }
 
+// The LDG launch of the boundary kernel whose arguments are q (p: q's BoundaryArgs): packed or dense known bits,
+// 4- or 1-wide vectors.  ldg_kernel names each kernel by its Args struct.
+template <int N, typename H, bool kPk>
+constexpr auto ldg_kernel(const BoundaryArgs&) { return boundary_kernel<N, H, kPk>; }
+
+template <typename H, typename A>
+int launch_ldg(const A& q, const BoundaryArgs& p, bool v4, cudaStream_t s) {
+  const dim3 grid(blocks_for(v4 ? p.g.total / 4 : p.g.total));
+  if (p.kwords) launch_kernel(v4 ? ldg_kernel<4, H, true>(q) : ldg_kernel<1, H, true>(q), grid, s, q);
+  else launch_kernel(v4 ? ldg_kernel<4, H, false>(q) : ldg_kernel<1, H, false>(q), grid, s, q);
+  return check_launch();
+}
+
+template <typename A>
+int launch_ldg(const A& q, const BoundaryArgs& p, int dtype, bool v4, cudaStream_t s) {
+  switch (dtype) {
+    case LP_DTYPE_F32: return launch_ldg<float>(q, p, v4, s);
+    case LP_DTYPE_BF16: return launch_ldg<__nv_bfloat16>(q, p, v4, s);
+    default: return launch_ldg<__half>(q, p, v4, s);
+  }
+}
+
 template <typename H>
-int boundary_dispatch(const BoundaryArgs& p, bool v4, int dtype, cudaStream_t s) {
+int boundary_dispatch(const BoundaryArgs& p, bool v4, cudaStream_t s) {
   const bool tma = v4 && g_opt_tma != 0 && g_opt_tma_boundary != 0 && p.x && geometry_tma(p.g, p.mask) && p.g.total >= (uint32_t)g_opt_tma_min &&
                    aligned16(p.a) && (!p.combine || aligned16(p.b)) && aligned16(p.y) && aligned16(p.x) &&
                    (!p.next_table || aligned16(p.noise)) && (!p.out || aligned16(p.out));
@@ -286,14 +349,7 @@ int boundary_dispatch(const BoundaryArgs& p, bool v4, int dtype, cudaStream_t s)
     if (p.next_table) return launch_boundary_tma<H, false, true>(p, s);
     return launch_boundary_tma<H, false, false>(p, s);
   }
-  if (p.kwords) {
-    if (v4) launch_kernel(boundary_kernel<4, H, true>, dim3(blocks_for(p.g.total / 4)), s, p);
-    else launch_kernel(boundary_kernel<1, H, true>, dim3(blocks_for(p.g.total)), s, p);
-  } else {
-    if (v4) launch_kernel(boundary_kernel<4, H, false>, dim3(blocks_for(p.g.total / 4)), s, p);
-    else launch_kernel(boundary_kernel<1, H, false>, dim3(blocks_for(p.g.total)), s, p);
-  }
-  return check_launch();
+  return launch_ldg<H>(p, p, v4, s);
 }
 
 // what every boundary entry point rejects, before any CUDA call
@@ -309,38 +365,61 @@ static int boundary_check(const lp_heads* mo, const float* y, const float* noise
   return LP_OK;
 }
 
-// the operands of a checked call whose geometry p.g is made
-static void boundary_args(BoundaryArgs& p, const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
-                          const lp_known* known, float* x_inout, float* out, float euler_coef,
-                          const float* next_table) {
-  p.a = mo->a; p.b = mo->combine ? mo->b : nullptr; p.y = y; p.noise = noise; p.mask = mask; p.x = x_inout; p.out = out;
+// Whether two of `bufs` -- fp32 buffers of `bytes` each, NULL entries absent -- share a byte.  A pair from the first
+// `k` is exempt: the launch lets those alias, and with `whole` they may be one buffer but must not overlap in part
+// (each element is read and written by one thread).
+static bool aliased(std::initializer_list<const void*> bufs, size_t bytes, size_t k, bool whole) {
+  const void* const* v = bufs.begin();
+  for (size_t m = 1; m < bufs.size(); ++m)
+    for (size_t l = 0; l < m; ++l) {
+      if (!v[m] || !v[l]) continue;
+      const uintptr_t u = reinterpret_cast<uintptr_t>(v[m]), w = reinterpret_cast<uintptr_t>(v[l]);
+      const bool shared = u == w || (u < w + bytes && w < u + bytes);
+      if (m < k ? whole && shared && u != w : shared) return true;
+    }
+  return false;
+}
+
+// The setup every boundary entry point shares, before any CUDA call: the checks (the sampler's own are `valid`), the
+// geometry, the aliasing rule on `states` (every fp32 buffer the launch reads or writes besides y and the noise, see
+// aliased), the operands, whether the heads' lines may be dropped and whether the launch runs 4-wide.  An empty
+// launch returns LP_OK with p.g.total == 0.
+static int boundary_setup(BoundaryArgs& p, bool& v4, bool valid, const lp_heads* mo, const float* y, const float* noise,
+                          const uint8_t* mask, const lp_known* known, float* x, float* out, float euler_coef,
+                          const float* next_table, const lp_dims* dims, std::initializer_list<const void*> states,
+                          size_t k, bool whole = false) {
+  v4 = false;
+  if (int rc = boundary_check(mo, y, noise, mask, known, x, out, next_table)) return rc;
+  if (!valid) return LP_ERR_INVALID;
+  if (int rc = make_geometry(dims, p.g)) return rc;
+  if (aliased(states, (size_t)p.g.total * sizeof(float), k, whole)) return LP_ERR_INVALID;
+  if (p.g.total == 0) return LP_OK;
+  p.a = mo->a; p.b = mo->combine ? mo->b : nullptr; p.y = y; p.noise = noise; p.mask = mask; p.x = x; p.out = out;
   p.kwords = known ? known->words : nullptr; p.yk = known ? known->y : nullptr; p.nk = known ? known->noise : nullptr;
   p.next_table = next_table; p.cfg = mo->cfg; p.coef = euler_coef; p.combine = mo->combine != 0;
   p.l2 = l2_handoff(p.g.total);
-  p.discard = heads_discard(mo, p.b, p.g.total, {x_inout, out});
-}
-
-static bool boundary_vec4(const BoundaryArgs& p, int dtype) {
-  return geometry_vec4(p.g, p.mask) && head_aligned(p.a, dtype) && (!p.b || head_aligned(p.b, dtype)) &&
-         aligned16(p.y) && (!p.noise || aligned16(p.noise)) && (!p.x || aligned16(p.x)) &&
-         (!p.out || aligned16(p.out));
+  p.discard = heads_discard(mo, p.b, p.g.total, states);  // a dropped line holds no state
+  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
+  v4 = geometry_vec4(p.g, p.mask) && head_aligned(p.a, dtype) && (!p.b || head_aligned(p.b, dtype)) &&
+       aligned16(p.y) && (!p.noise || aligned16(p.noise));
+  for (const void* b : states) v4 = v4 && (!b || aligned16(b));
+  return LP_OK;
 }
 
 static int boundary_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
                          const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
                          const lp_dims* dims, lp_stream_t stream) {
-  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
   BoundaryArgs p;
-  if (int rc = make_geometry(dims, p.g)) return rc;
+  bool v4;
+  if (int rc = boundary_setup(p, v4, true, mo, y, noise, mask, known, x_inout, out, euler_coef, next_table, dims,
+                              {x_inout, out}, 2))
+    return rc;
   if (p.g.total == 0) return LP_OK;
-  boundary_args(p, mo, y, noise, mask, known, x_inout, out, euler_coef, next_table);
-  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
-  const bool v4 = boundary_vec4(p, dtype);
   cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case LP_DTYPE_F32: return boundary_dispatch<float>(p, v4, dtype, s);
-    case LP_DTYPE_BF16: return boundary_dispatch<__nv_bfloat16>(p, v4, dtype, s);
-    default: return boundary_dispatch<__half>(p, v4, dtype, s);
+  switch (mo->dtype & ~LP_HEADS_DEAD) {
+    case LP_DTYPE_F32: return boundary_dispatch<float>(p, v4, s);
+    case LP_DTYPE_BF16: return boundary_dispatch<__nv_bfloat16>(p, v4, s);
+    default: return boundary_dispatch<__half>(p, v4, s);
   }
 }
 
@@ -359,85 +438,39 @@ struct AncestralArgs {
   uint32_t torch_T;  // threads of torch's randn grid (LP_RNG_TORCH)
 };
 
-// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; x += ((x - o) / sigma) down ;
-// x += (xi s_noise) sigma_up ; x = known ? rn n + ry y : x
+// x += ((x - o) / sigma) down ; x += (xi s_noise) sigma_up
+__device__ __forceinline__ void ancestral_update(float& x, float o, const lp_ancestral& st, bool draw, float xi) {
+  x = __fadd_rn(x, __fmul_rn(__fdiv_rn(__fsub_rn(x, o), st.sigma), st.down));
+  if (draw) x = __fadd_rn(x, __fmul_rn(__fmul_rn(xi, st.s_noise), st.sigma_up));
+}
+
+// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; ancestral_update ; x = known ? rn n + ry y : x
 __device__ __forceinline__ void ancestral_element(float a, float b, float y, float nz, bool known, float& x, float& o,
                                                   bool combine, float cfg, const lp_ancestral& st, bool draw, float xi,
                                                   bool next, float rn, float ry) {
   const float d = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
   o = known ? y : d;
-  x = __fadd_rn(x, __fmul_rn(__fdiv_rn(__fsub_rn(x, o), st.sigma), st.down));
-  if (draw) x = __fadd_rn(x, __fmul_rn(__fmul_rn(xi, st.s_noise), st.sigma_up));
+  ancestral_update(x, o, st, draw, xi);
   if (next) x = known ? fmaf(rn, nz, ry * y) : x;  // rounds as prologue_kernel does
 }
 
-// one N-wide vector: the operand loads of boundary_kernel, x always updated
-template <int N, typename H, bool kPk>
-__device__ __forceinline__ void ancestral_vector(const AncestralArgs& q, uint32_t i, const float (&xi)[N], bool draw) {
-  const BoundaryArgs& p = q.b;
-  const uint64_t dead = l2_policy_dead(p.l2);
-  uint32_t row, mi;
-  locate(p.g, i, row, mi);
-  const bool next = p.next_table != nullptr;
-  float av[N], bv[N], yv[N], xv[N], nv[N], ov[N];
-  bool known[N];
-  uint32_t kb = 0, kidx = 0;
-  if constexpr (kPk) {
-    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
-    if constexpr (N == 4) {
-      known_quad(w, i, kb, kidx);
-    } else {
-      kb = (w.x >> (i & 31u)) & 1u;
-      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
-    }
-#pragma unroll
-    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
-  } else {
-    load_m<N>(p.mask, mi, known);
+// boundary_ancestral_kernel: x always read (where its update survives) and written.  No discard: with LP_RNG_TORCH a
+// warp's elements are not one contiguous span, so a warp-span discard would drop lines other warps still read.
+template <int N, bool kDraw>
+struct AncestralUpdate {
+  static constexpr bool kDiscard = false;
+  const AncestralArgs& q;
+  float xi[N];  // the sampler's randn_like at the vector's elements
+  float xv[N] = {};
+  __device__ __forceinline__ void load(uint32_t i, bool update, uint64_t) {
+    if (update) load_f<N>(q.b.x, i, xv);
   }
-  bool any_known = false, any_free = false;
-#pragma unroll
-  for (int j = 0; j < N; ++j) {
-    any_known |= known[j];
-    any_free |= !known[j];
+  __device__ __forceinline__ float& update(int j, float o) {
+    ancestral_update(xv[j], o, q.st, kDraw, xi[j]);
+    return xv[j];
   }
-#pragma unroll
-  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = 0.f;
-  if constexpr (kPk) {
-    if constexpr (N == 4) {
-      gather_known4<false>(p.yk, kb, kidx, yv);
-    } else {
-      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
-    }
-  } else {
-    load_f_ro<N>(p.y, i, yv);
-  }
-  if (any_free) {
-    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
-    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
-  }
-  if (any_free || !next) load_f<N>(p.x, i, xv);
-  float rn = 0.f, ry = 0.f;
-  if (next) {
-    if constexpr (kPk) {
-      if constexpr (N == 4) {
-        gather_known4<false>(p.nk, kb, kidx, nv);
-      } else {
-        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
-      }
-    } else {
-      if (any_known) load_f_ro<N>(p.noise, i, nv);
-    }
-    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
-    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j)
-    ancestral_element(av[j], bv[j], yv[j], nv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st, draw, xi[j], next,
-                      rn, ry);
-  if (p.out) store_f<N>(p.out, i, ov, dead);
-  store_f<N>(p.x, i, xv);
-}
+  __device__ __forceinline__ void store(uint32_t i) { store_f<N>(q.b.x, i, xv); }
+};
 
 // LDG form: small or ragged launches, and the TAPE / PHILOX streams.  LP_RNG_TORCH maps threads onto torch's own
 // randn grid: N == 4 as substep_torchvec_kernel does (thread (t, k) draws call k of subsequence t, a quad transposes
@@ -457,11 +490,11 @@ __global__ void __launch_bounds__(kBlock) boundary_ancestral_kernel(const Ancest
     if constexpr (N == 4) {
       const uint32_t k = blockIdx.y, l = t & 3u;
       const float4 n = torch_normal4(seed, o0, t, k);
-      float xi[4] = {n.x, n.y, n.z, n.w};
-      quad_transpose(xi, l);
+      AncestralUpdate<4, true> u{q, {n.x, n.y, n.z, n.w}};
+      quad_transpose(u.xi, l);
       const uint64_t e = (uint64_t)(t - l) + (uint64_t)(4u * k + l) * T;  // first of my 4 consecutive elements
       if (e >= total) return;
-      ancestral_vector<4, H, kPk>(q, (uint32_t)e, xi, true);
+      boundary_vector<4, H, kPk>(q.b, (uint32_t)e, u);
     } else {
       if (t >= T) return;
       uint32_t call = 0;
@@ -471,17 +504,16 @@ __global__ void __launch_bounds__(kBlock) boundary_ancestral_kernel(const Ancest
         for (int ii = 0; ii < 4; ++ii) {
           const uint64_t li = base + (uint64_t)ii * T;
           if (li >= total) break;
-          const float xi[1] = {pick(n, ii)};
-          ancestral_vector<1, H, kPk>(q, (uint32_t)li, xi, true);
+          AncestralUpdate<1, true> u{q, {pick(n, ii)}};
+          boundary_vector<1, H, kPk>(q.b, (uint32_t)li, u);
         }
       }
     }
   } else {
     const uint32_t i = (walk_index(q.b.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
     if (i >= total) return;
-    float xi[N];
-#pragma unroll
-    for (int j = 0; j < N; ++j) xi[j] = 0.f;
+    AncestralUpdate<N, kRng != kRngNone> u{q, {}};
+    float(&xi)[N] = u.xi;
     if constexpr (kRng == LP_RNG_TAPE) {
       load_f_ro<N>(q.tape0, i, xi);
     } else if constexpr (kRng == LP_RNG_PHILOX) {
@@ -497,7 +529,7 @@ __global__ void __launch_bounds__(kBlock) boundary_ancestral_kernel(const Ancest
         xi[0] = pick(n, i & 3);
       }
     }
-    ancestral_vector<N, H, kPk>(q, i, xi, kRng != kRngNone);
+    boundary_vector<N, H, kPk>(q.b, i, u);
   }
 }
 
@@ -773,29 +805,24 @@ static int boundary_ancestral_impl(const lp_heads* mo, const float* y, const flo
                                    const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
                                    const lp_rng* rng, const float* next_table, const lp_dims* dims,
                                    lp_stream_t stream) {
-  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
-  if (!x_inout || !step || !(step->sigma > 0.f)) return LP_ERR_INVALID;
-  if (!rng && step->sigma_up != 0.f) return LP_ERR_INVALID;
-  int mode = kRngNone;
-  if (rng) {
-    mode = rng->mode;
-    if (mode != LP_RNG_TAPE && mode != LP_RNG_PHILOX && mode != LP_RNG_TORCH) return LP_ERR_INVALID;
-    if (mode == LP_RNG_TAPE && !rng->tape0) return LP_ERR_INVALID;
-  }
+  const int mode = rng ? rng->mode : kRngNone;
+  const bool valid = x_inout && step && step->sigma > 0.f && (rng || step->sigma_up == 0.f) &&
+                     (!rng || mode == LP_RNG_TAPE || mode == LP_RNG_PHILOX || mode == LP_RNG_TORCH) &&
+                     (mode != LP_RNG_TAPE || rng->tape0);
   AncestralArgs q;
-  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  bool v4;
+  if (int rc = boundary_setup(q.b, v4, valid, mo, y, noise, mask, known, x_inout, out, 0.f, next_table, dims,
+                              {x_inout, out}, 2))
+    return rc;
   if (q.b.g.total == 0) return LP_OK;
-  boundary_args(q.b, mo, y, noise, mask, known, x_inout, out, 0.f, next_table);
   q.st = *step;
   q.tape0 = rng ? rng->tape0 : nullptr;
   q.rng_state = rng ? rng->state : nullptr;
   q.seed = rng ? rng->seed : 0;
   q.draw0 = rng ? rng->draw0 : 0;
   q.torch_T = 0;
-  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
-  const bool v4 = boundary_vec4(q.b, dtype);
   cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
+  switch (mo->dtype & ~LP_HEADS_DEAD) {
     case LP_DTYPE_F32: return ancestral_dispatch<float>(q, mode, v4, s);
     case LP_DTYPE_BF16: return ancestral_dispatch<__nv_bfloat16>(q, mode, v4, s);
     default: return ancestral_dispatch<__half>(q, mode, v4, s);
@@ -812,145 +839,50 @@ struct MultistepArgs {
   const float* old;  // the previous step's out; NULL: first-order step
 };
 
-// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; dd = old ? c_cur o - c_old old : o ;
-// x = ratio x - em1 dd ; x = known ? rn n + ry y : x
-__device__ __forceinline__ void multistep_element(float a, float b, float y, float nz, float old, bool known, float& x,
-                                                  float& o, bool combine, float cfg, const lp_multistep& st,
-                                                  bool second, bool next, float rn, float ry) {
-  const float d = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
-  o = known ? y : d;
-  const float dd = second ? __fsub_rn(__fmul_rn(st.c_cur, o), __fmul_rn(st.c_old, old)) : o;
-  x = __fsub_rn(__fmul_rn(st.ratio, x), __fmul_rn(st.em1, dd));
-  if (next) x = known ? fmaf(rn, nz, ry * y) : x;  // rounds as prologue_kernel does
-}
+// dd = old ? c_cur o - c_old old : o ; x = ratio x - em1 dd ; x and old read where x's update survives
+template <int N>
+struct MultistepUpdate {
+  static constexpr bool kDiscard = true;
+  const MultistepArgs& q;
+  float xv[N] = {}, dv[N] = {};
+  __device__ __forceinline__ void load(uint32_t i, bool update, uint64_t dead) {
+    if (update) load_f<N>(q.b.x, i, xv);
+    if (q.old && update) load_head_ro<N, float>(q.old, i, dv, dead);  // nothing reads the previous out again
+  }
+  __device__ __forceinline__ float& update(int j, float o) {
+    const float dd = q.old ? __fsub_rn(__fmul_rn(q.st.c_cur, o), __fmul_rn(q.st.c_old, dv[j])) : o;
+    xv[j] = __fsub_rn(__fmul_rn(q.st.ratio, xv[j]), __fmul_rn(q.st.em1, dd));
+    return xv[j];
+  }
+  __device__ __forceinline__ void store(uint32_t i) { store_f<N>(q.b.x, i, xv); }
+};
 
-// boundary_kernel's form and operand skipping, x always updated; old is read where x's update survives
 template <int N, typename H, bool kPk>
 __global__ void __launch_bounds__(kBlock) boundary_multistep_kernel(const MultistepArgs q) {
   pdl_prologue();
-  const BoundaryArgs& p = q.b;
-  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
-  if (i >= p.g.total) return;
-  const uint64_t dead = l2_policy_dead(p.l2);
-  uint32_t row, mi;
-  locate(p.g, i, row, mi);
-  const bool next = p.next_table != nullptr, second = q.old != nullptr;
-  float av[N], bv[N], yv[N], xv[N], nv[N], dv[N], ov[N];
-  bool known[N];
-  uint32_t kb = 0, kidx = 0;
-  if constexpr (kPk) {
-    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
-    if constexpr (N == 4) {
-      known_quad(w, i, kb, kidx);
-    } else {
-      kb = (w.x >> (i & 31u)) & 1u;
-      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
-    }
-#pragma unroll
-    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
-  } else {
-    load_m<N>(p.mask, mi, known);
-  }
-  bool any_known = false, any_free = false;
-#pragma unroll
-  for (int j = 0; j < N; ++j) {
-    any_known |= known[j];
-    any_free |= !known[j];
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = dv[j] = 0.f;
-  if constexpr (kPk) {
-    if constexpr (N == 4) {
-      gather_known4<false>(p.yk, kb, kidx, yv);
-    } else {
-      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
-    }
-  } else {
-    load_f_ro<N>(p.y, i, yv);
-  }
-  if (any_free) {
-    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
-    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
-  }
-  const bool update = any_free || !next;  // somewhere in the vector x's update is not overwritten by the replace step
-  if (update) load_f<N>(p.x, i, xv);
-  if (second && update) load_head_ro<N, float>(q.old, i, dv, dead);  // nothing reads the previous out again
-  float rn = 0.f, ry = 0.f;
-  if (next) {
-    if constexpr (kPk) {
-      if constexpr (N == 4) {
-        gather_known4<false>(p.nk, kb, kidx, nv);
-      } else {
-        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
-      }
-    } else {
-      if (any_known) load_f_ro<N>(p.noise, i, nv);
-    }
-    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
-    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j)
-    multistep_element(av[j], bv[j], yv[j], nv[j], dv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st, second,
-                      next, rn, ry);
-  if (p.out) store_f<N>(p.out, i, ov, dead);
-  store_f<N>(p.x, i, xv);
-  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
-    if (p.discard) {
-      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
-      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
-        __syncwarp();           // every lane's head loads are used
-        discard_line<H>(p.a, i, end);
-        if (p.b) discard_line<H>(p.b, i, end);
-      }
-    }
-  }
+  const uint32_t i = (walk_index(q.b.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= q.b.g.total) return;
+  MultistepUpdate<N> u{q};
+  boundary_vector<N, H, kPk>(q.b, i, u);
 }
 
-template <typename H>
-int multistep_dispatch(const MultistepArgs& q, bool v4, cudaStream_t s) {
-  const uint32_t total = q.b.g.total;
-  if (q.b.kwords) {
-    if (v4) launch_kernel(boundary_multistep_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_multistep_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
-  } else {
-    if (v4) launch_kernel(boundary_multistep_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_multistep_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
-  }
-  return check_launch();
-}
-
-static bool overlaps(const void* p, const void* q, size_t bytes) {
-  const uintptr_t u = reinterpret_cast<uintptr_t>(p), v = reinterpret_cast<uintptr_t>(q);
-  return u < v + bytes && v < u + bytes;
-}
+template <int N, typename H, bool kPk>
+constexpr auto ldg_kernel(const MultistepArgs&) { return boundary_multistep_kernel<N, H, kPk>; }
 
 static int boundary_multistep_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
                                    const lp_known* known, float* x_inout, float* out, const float* old_out,
                                    const lp_multistep* step, const float* next_table, const lp_dims* dims,
                                    lp_stream_t stream) {
-  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
-  if (!x_inout || !step) return LP_ERR_INVALID;
   MultistepArgs q;
-  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  bool v4;
   // the launch writes x and out while it reads old_out
-  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
-  if (old_out && (old_out == x_inout || old_out == out || overlaps(old_out, x_inout, bytes) ||
-                  (out && overlaps(old_out, out, bytes))))
-    return LP_ERR_INVALID;
+  if (int rc = boundary_setup(q.b, v4, x_inout && step, mo, y, noise, mask, known, x_inout, out, 0.f, next_table, dims,
+                              {x_inout, out, old_out}, 2))
+    return rc;
   if (q.b.g.total == 0) return LP_OK;
-  boundary_args(q.b, mo, y, noise, mask, known, x_inout, out, 0.f, next_table);
-  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x_inout, out, old_out});  // a dropped line must hold no old_out
   q.st = *step;
   q.old = old_out;
-  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
-  const bool v4 = boundary_vec4(q.b, dtype) && (!old_out || aligned16(old_out));
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case LP_DTYPE_F32: return multistep_dispatch<float>(q, v4, s);
-    case LP_DTYPE_BF16: return multistep_dispatch<__nv_bfloat16>(q, v4, s);
-    default: return multistep_dispatch<__half>(q, v4, s);
-  }
+  return launch_ldg(q, q.b, mo->dtype & ~LP_HEADS_DEAD, v4, (cudaStream_t)stream);
 }
 
 // ---- the boundary of a wrapper call of a host-owned DPM-Solver-2 loop ------------------------------------------
@@ -965,66 +897,14 @@ struct MidpointArgs {
   int evict;            // x_in / x_base are not read again before a whole network call: load them evict-first
 };
 
-// per element: d = combine ? b + (a-b) cfg : a ; o = known ? y : d ; x = base + ((in - o) / sigma) dt ;
-// x = known ? rn n + ry y : x
-__device__ __forceinline__ void midpoint_element(float a, float b, float y, float nz, float in, float base, bool known,
-                                                 float& x, float& o, bool combine, float cfg, const lp_midpoint& st,
-                                                 bool next, float rn, float ry) {
-  const float d = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
-  o = known ? y : d;
-  x = __fadd_rn(base, __fmul_rn(__fdiv_rn(__fsub_rn(in, o), st.sigma), st.dt));
-  if (next) x = known ? fmaf(rn, nz, ry * y) : x;  // rounds as prologue_kernel does
-}
-
-// boundary_kernel's form and operand skipping; x_in and x_base are read where x_out's update survives
-template <int N, typename H, bool kPk>
-__global__ void __launch_bounds__(kBlock) boundary_midpoint_kernel(const MidpointArgs q) {
-  pdl_prologue();
-  const BoundaryArgs& p = q.b;
-  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
-  if (i >= p.g.total) return;
-  const uint64_t dead = l2_policy_dead(p.l2);
-  uint32_t row, mi;
-  locate(p.g, i, row, mi);
-  const bool next = p.next_table != nullptr;
-  float av[N], bv[N], yv[N], nv[N], iv[N], sv[N], xv[N], ov[N];
-  bool known[N];
-  uint32_t kb = 0, kidx = 0;
-  if constexpr (kPk) {
-    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
-    if constexpr (N == 4) {
-      known_quad(w, i, kb, kidx);
-    } else {
-      kb = (w.x >> (i & 31u)) & 1u;
-      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
-    }
-#pragma unroll
-    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
-  } else {
-    load_m<N>(p.mask, mi, known);
-  }
-  bool any_known = false, any_free = false;
-#pragma unroll
-  for (int j = 0; j < N; ++j) {
-    any_known |= known[j];
-    any_free |= !known[j];
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j) av[j] = bv[j] = nv[j] = iv[j] = sv[j] = 0.f;
-  if constexpr (kPk) {
-    if constexpr (N == 4) {
-      gather_known4<false>(p.yk, kb, kidx, yv);
-    } else {
-      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
-    }
-  } else {
-    load_f_ro<N>(p.y, i, yv);
-  }
-  if (any_free) {
-    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
-    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
-  }
-  if (any_free || !next) {  // somewhere in the vector x_out's update is not overwritten by the replace step
+// x_out = base + ((in - o) / sigma) dt ; x_in and x_base read where x_out's update survives, x_out not read
+template <int N>
+struct MidpointUpdate {
+  static constexpr bool kDiscard = true;
+  const MidpointArgs& q;
+  float iv[N] = {}, sv[N] = {}, xv[N];
+  __device__ __forceinline__ void load(uint32_t i, bool update, uint64_t dead) {
+    if (!update) return;
     const uint64_t xp = q.evict ? dead : 0;
     load_f<N>(q.xin, i, iv, xp);
     if (q.xbase != q.xin) {
@@ -1034,81 +914,44 @@ __global__ void __launch_bounds__(kBlock) boundary_midpoint_kernel(const Midpoin
       for (int j = 0; j < N; ++j) sv[j] = iv[j];
     }
   }
-  float rn = 0.f, ry = 0.f;
-  if (next) {
-    if constexpr (kPk) {
-      if constexpr (N == 4) {
-        gather_known4<false>(p.nk, kb, kidx, nv);
-      } else {
-        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
-      }
-    } else {
-      if (any_known) load_f_ro<N>(p.noise, i, nv);
-    }
-    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
-    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+  __device__ __forceinline__ float& update(int j, float o) {
+    xv[j] = __fadd_rn(sv[j], __fmul_rn(__fdiv_rn(__fsub_rn(iv[j], o), q.st.sigma), q.st.dt));
+    return xv[j];
   }
-#pragma unroll
-  for (int j = 0; j < N; ++j)
-    midpoint_element(av[j], bv[j], yv[j], nv[j], iv[j], sv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st,
-                     next, rn, ry);
-  if (p.out) store_f<N>(p.out, i, ov, dead);
-  store_f<N>(p.x, i, xv);  // normal policy: the next network call reads x_out first
-  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
-    if (p.discard) {
-      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
-      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
-        __syncwarp();           // every lane's head loads are used
-        discard_line<H>(p.a, i, end);
-        if (p.b) discard_line<H>(p.b, i, end);
-      }
-    }
+  __device__ __forceinline__ void store(uint32_t i) {
+    store_f<N>(q.b.x, i, xv);  // normal policy: the next network call reads x_out first
   }
+};
+
+template <int N, typename H, bool kPk>
+__global__ void __launch_bounds__(kBlock) boundary_midpoint_kernel(const MidpointArgs q) {
+  pdl_prologue();
+  const uint32_t i = (walk_index(q.b.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= q.b.g.total) return;
+  MidpointUpdate<N> u{q};
+  boundary_vector<N, H, kPk>(q.b, i, u);
 }
 
-template <typename H>
-int midpoint_dispatch(const MidpointArgs& q, bool v4, cudaStream_t s) {
-  const uint32_t total = q.b.g.total;
-  if (q.b.kwords) {
-    if (v4) launch_kernel(boundary_midpoint_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_midpoint_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
-  } else {
-    if (v4) launch_kernel(boundary_midpoint_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_midpoint_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
-  }
-  return check_launch();
-}
+template <int N, typename H, bool kPk>
+constexpr auto ldg_kernel(const MidpointArgs&) { return boundary_midpoint_kernel<N, H, kPk>; }
 
 static int boundary_midpoint_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
                                   const lp_known* known, const float* x_in, const float* x_base, float* x_out,
                                   float* out, const lp_midpoint* step, const float* next_table, const lp_dims* dims,
                                   lp_stream_t stream) {
-  if (int rc = boundary_check(mo, y, noise, mask, known, x_out, out, next_table)) return rc;
-  if (!step || !x_in || !x_base || !x_out) return LP_ERR_INVALID;
   MidpointArgs q;
-  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  bool v4;
   // one thread reads and writes each element: the three states are each one buffer or disjoint, and out, which the
   // launch writes, shares no byte with any of them
-  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
-  const auto partial = [&](const void* u, const void* v) { return u != v && overlaps(u, v, bytes); };
-  const auto any = [&](const void* u, const void* v) { return u == v || overlaps(u, v, bytes); };
-  if (partial(x_in, x_base) || partial(x_in, x_out) || partial(x_base, x_out)) return LP_ERR_INVALID;
-  if (out && (any(out, x_in) || any(out, x_base) || any(out, x_out))) return LP_ERR_INVALID;
+  if (int rc = boundary_setup(q.b, v4, step && x_in && x_base && x_out, mo, y, noise, mask, known, x_out, out, 0.f,
+                              next_table, dims, {x_in, x_base, x_out, out}, 3, true))
+    return rc;
   if (q.b.g.total == 0) return LP_OK;
-  boundary_args(q.b, mo, y, noise, mask, known, x_out, out, 0.f, next_table);
-  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x_in, x_base, x_out, out});  // a dropped line holds no state
   q.st = *step;
   q.xin = x_in;
   q.xbase = x_base;
   q.evict = !(x_in == x_out && x_base == x_out);  // the predictor's X, the corrector's X2 and X
-  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
-  const bool v4 = boundary_vec4(q.b, dtype) && aligned16(x_in) && aligned16(x_base);
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case LP_DTYPE_F32: return midpoint_dispatch<float>(q, v4, s);
-    case LP_DTYPE_BF16: return midpoint_dispatch<__nv_bfloat16>(q, v4, s);
-    default: return midpoint_dispatch<__half>(q, v4, s);
-  }
+  return launch_ldg(q, q.b, mo->dtype & ~LP_HEADS_DEAD, v4, (cudaStream_t)stream);
 }
 
 // ---- the boundary of an outer step of a host-owned DEIS loop ---------------------------------------------------
@@ -1123,153 +966,62 @@ struct DeisArgs {
   const float* p2;     // the one before it; NULL: first or second order
 };
 
-// per element: den = combine ? b + (a-b) cfg : a ; o = known ? y : den ; d = (x - o) / sigma ;
-// x = x + c_cur d [+ c_prev1 p1 [+ c_prev2 p2]] ; x = known ? rn n + ry y : x
-__device__ __forceinline__ void deis_element(float a, float b, float y, float nz, float p1, float p2, bool known,
-                                             float& x, float& o, float& d, bool combine, float cfg, const lp_deis& st,
-                                             bool second, bool third, bool next, float rn, float ry) {
-  const float den = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
-  o = known ? y : den;
-  d = __fdiv_rn(__fsub_rn(x, o), st.sigma);
-  float u = __fadd_rn(x, __fmul_rn(st.c_cur, d));
-  if (second) u = __fadd_rn(u, __fmul_rn(st.c_prev1, p1));
-  if (third) u = __fadd_rn(u, __fmul_rn(st.c_prev2, p2));
-  x = next && known ? fmaf(rn, nz, ry * y) : u;  // the replace step rounds as prologue_kernel does
-}
+// d = (x - o) / sigma ; x = x + c_cur d [+ c_prev1 p1 [+ c_prev2 p2]] ; the history read where x's update survives,
+// x also where d is written at a known position
+template <int N>
+struct DeisUpdate {
+  static constexpr bool kDiscard = true;
+  const DeisArgs& q;
+  const bool second = q.p1 != nullptr, third = q.p2 != nullptr;
+  float xv[N] = {}, v1[N] = {}, v2[N] = {}, dv[N];
+  __device__ __forceinline__ void load(uint32_t i, bool update, uint64_t dead) {
+    if (update || q.dout) load_f<N>(q.b.x, i, xv);
+    if (second && update) load_f_ro<N>(q.p1, i, v1);                  // the next step reads it again, as its d_prev2
+    if (third && update) load_head_ro<N, float>(q.p2, i, v2, dead);   // nothing reads it again
+  }
+  __device__ __forceinline__ float& update(int j, float o) {
+    dv[j] = __fdiv_rn(__fsub_rn(xv[j], o), q.st.sigma);
+    float u = __fadd_rn(xv[j], __fmul_rn(q.st.c_cur, dv[j]));
+    if (second) u = __fadd_rn(u, __fmul_rn(q.st.c_prev1, v1[j]));
+    if (third) u = __fadd_rn(u, __fmul_rn(q.st.c_prev2, v2[j]));
+    xv[j] = u;
+    return xv[j];
+  }
+  __device__ __forceinline__ void store(uint32_t i) {
+    if (q.dout) store_f<N>(q.dout, i, dv);  // normal policy: the next step reads it
+    store_f<N>(q.b.x, i, xv);
+  }
+};
 
-// boundary_kernel's form and operand skipping; the history is read where x's update survives, x also where d is
-// written at a known position
 template <int N, typename H, bool kPk>
 __global__ void __launch_bounds__(kBlock) boundary_deis_kernel(const DeisArgs q) {
   pdl_prologue();
-  const BoundaryArgs& p = q.b;
-  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
-  if (i >= p.g.total) return;
-  const uint64_t dead = l2_policy_dead(p.l2);
-  uint32_t row, mi;
-  locate(p.g, i, row, mi);
-  const bool next = p.next_table != nullptr, second = q.p1 != nullptr, third = q.p2 != nullptr;
-  float av[N], bv[N], yv[N], xv[N], nv[N], v1[N], v2[N], ov[N], dv[N];
-  bool known[N];
-  uint32_t kb = 0, kidx = 0;
-  if constexpr (kPk) {
-    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
-    if constexpr (N == 4) {
-      known_quad(w, i, kb, kidx);
-    } else {
-      kb = (w.x >> (i & 31u)) & 1u;
-      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
-    }
-#pragma unroll
-    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
-  } else {
-    load_m<N>(p.mask, mi, known);
-  }
-  bool any_known = false, any_free = false;
-#pragma unroll
-  for (int j = 0; j < N; ++j) {
-    any_known |= known[j];
-    any_free |= !known[j];
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = v1[j] = v2[j] = 0.f;
-  if constexpr (kPk) {
-    if constexpr (N == 4) {
-      gather_known4<false>(p.yk, kb, kidx, yv);
-    } else {
-      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
-    }
-  } else {
-    load_f_ro<N>(p.y, i, yv);
-  }
-  if (any_free) {
-    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
-    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
-  }
-  const bool update = any_free || !next;  // somewhere in the vector x's update is not overwritten by the replace step
-  if (update || q.dout) load_f<N>(p.x, i, xv);
-  if (second && update) load_f_ro<N>(q.p1, i, v1);                  // the next step reads it again, as its d_prev2
-  if (third && update) load_head_ro<N, float>(q.p2, i, v2, dead);   // nothing reads it again
-  float rn = 0.f, ry = 0.f;
-  if (next) {
-    if constexpr (kPk) {
-      if constexpr (N == 4) {
-        gather_known4<false>(p.nk, kb, kidx, nv);
-      } else {
-        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
-      }
-    } else {
-      if (any_known) load_f_ro<N>(p.noise, i, nv);
-    }
-    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
-    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j)
-    deis_element(av[j], bv[j], yv[j], nv[j], v1[j], v2[j], known[j], xv[j], ov[j], dv[j], p.combine != 0, p.cfg, q.st,
-                 second, third, next, rn, ry);
-  if (p.out) store_f<N>(p.out, i, ov, dead);
-  if (q.dout) store_f<N>(q.dout, i, dv);  // normal policy: the next step reads it
-  store_f<N>(p.x, i, xv);
-  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
-    if (p.discard) {
-      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
-      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
-        __syncwarp();           // every lane's head loads are used
-        discard_line<H>(p.a, i, end);
-        if (p.b) discard_line<H>(p.b, i, end);
-      }
-    }
-  }
+  const uint32_t i = (walk_index(q.b.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= q.b.g.total) return;
+  DeisUpdate<N> u{q};
+  boundary_vector<N, H, kPk>(q.b, i, u);
 }
 
-template <typename H>
-int deis_dispatch(const DeisArgs& q, bool v4, cudaStream_t s) {
-  const uint32_t total = q.b.g.total;
-  if (q.b.kwords) {
-    if (v4) launch_kernel(boundary_deis_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_deis_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
-  } else {
-    if (v4) launch_kernel(boundary_deis_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_deis_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
-  }
-  return check_launch();
-}
+template <int N, typename H, bool kPk>
+constexpr auto ldg_kernel(const DeisArgs&) { return boundary_deis_kernel<N, H, kPk>; }
 
 static int boundary_deis_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
                               const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev1,
                               const float* d_prev2, const lp_deis* step, const float* next_table, const lp_dims* dims,
                               lp_stream_t stream) {
-  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
-  if (!x_inout || !step || (d_prev2 && !d_prev1)) return LP_ERR_INVALID;
   DeisArgs q;
-  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  bool v4;
   // the launch writes x, out and d_out while it reads the history: the three histories share no byte with each other
   // or with x and out
-  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
-  const auto any = [&](const void* u, const void* v) { return u && v && (u == v || overlaps(u, v, bytes)); };
-  const void* hist[3] = {d_out, d_prev1, d_prev2};
-  for (int k = 0; k < 3; ++k) {
-    if (any(hist[k], x_inout) || any(hist[k], out)) return LP_ERR_INVALID;
-    for (int l = 0; l < k; ++l)
-      if (any(hist[k], hist[l])) return LP_ERR_INVALID;
-  }
+  if (int rc = boundary_setup(q.b, v4, x_inout && step && (d_prev1 || !d_prev2), mo, y, noise, mask, known, x_inout,
+                              out, 0.f, next_table, dims, {x_inout, out, d_out, d_prev1, d_prev2}, 2))
+    return rc;
   if (q.b.g.total == 0) return LP_OK;
-  boundary_args(q.b, mo, y, noise, mask, known, x_inout, out, 0.f, next_table);
-  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x_inout, out, d_out, d_prev1, d_prev2});  // no state dropped
   q.st = *step;
   q.dout = d_out;
   q.p1 = d_prev1;
   q.p2 = d_prev2;
-  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
-  const bool v4 = boundary_vec4(q.b, dtype) && (!d_out || aligned16(d_out)) && (!d_prev1 || aligned16(d_prev1)) &&
-                  (!d_prev2 || aligned16(d_prev2));
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case LP_DTYPE_F32: return deis_dispatch<float>(q, v4, s);
-    case LP_DTYPE_BF16: return deis_dispatch<__nv_bfloat16>(q, v4, s);
-    default: return deis_dispatch<__half>(q, v4, s);
-  }
+  return launch_ldg(q, q.b, mo->dtype & ~LP_HEADS_DEAD, v4, (cudaStream_t)stream);
 }
 
 // ---- the boundary of an outer step of a host-owned gradient-estimation loop ---------------------------------------
@@ -1284,150 +1036,60 @@ struct GeArgs {
   const float* prev;   // the previous step's d; NULL: no correction
 };
 
-// per element: den = combine ? b + (a-b) cfg : a ; o = known ? y : den ; d = (x - o) / sigma ;
-// x = final ? o : x + d dt [+ (gm1 (d - prev)) dt] ; x = known ? rn n + ry y : x
-__device__ __forceinline__ void ge_element(float a, float b, float y, float nz, float pv, bool known, float& x,
-                                           float& o, float& d, bool combine, float cfg,
-                                           const lp_gradient_estimation& st, bool fin, bool hist, bool next, float rn,
-                                           float ry) {
-  const float den = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
-  o = known ? y : den;
-  d = __fdiv_rn(__fsub_rn(x, o), st.sigma);
-  float u = o;
-  if (!fin) {
-    u = __fadd_rn(x, __fmul_rn(d, st.dt));
-    if (hist) u = __fadd_rn(u, __fmul_rn(__fmul_rn(st.gm1, __fsub_rn(d, pv)), st.dt));
+// d = (x - o) / sigma ; x = final ? o : x + d dt [+ (gm1 (d - prev)) dt] ; the history read where x's update
+// survives, x where the update reads it or d is written
+template <int N>
+struct GeUpdate {
+  static constexpr bool kDiscard = true;
+  const GeArgs& q;
+  float xv[N] = {}, pv[N] = {}, dv[N];
+  __device__ __forceinline__ void load(uint32_t i, bool update, uint64_t dead) {
+    if ((update && !q.st.final) || q.dout) load_f<N>(q.b.x, i, xv);
+    if (q.prev && update) load_head_ro<N, float>(q.prev, i, pv, dead);  // nothing reads it again
   }
-  x = next && known ? fmaf(rn, nz, ry * y) : u;  // the replace step rounds as prologue_kernel does
-}
+  __device__ __forceinline__ float& update(int j, float o) {
+    dv[j] = __fdiv_rn(__fsub_rn(xv[j], o), q.st.sigma);
+    float u = o;
+    if (!q.st.final) {
+      u = __fadd_rn(xv[j], __fmul_rn(dv[j], q.st.dt));
+      if (q.prev) u = __fadd_rn(u, __fmul_rn(__fmul_rn(q.st.gm1, __fsub_rn(dv[j], pv[j])), q.st.dt));
+    }
+    xv[j] = u;
+    return xv[j];
+  }
+  __device__ __forceinline__ void store(uint32_t i) {
+    if (q.dout) store_f<N>(q.dout, i, dv);  // normal policy: the next step reads it
+    store_f<N>(q.b.x, i, xv);
+  }
+};
 
-// boundary_kernel's form and operand skipping; the history is read where x's update survives, x where the update
-// reads it or d is written
 template <int N, typename H, bool kPk>
 __global__ void __launch_bounds__(kBlock) boundary_ge_kernel(const GeArgs q) {
   pdl_prologue();
-  const BoundaryArgs& p = q.b;
-  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
-  if (i >= p.g.total) return;
-  const uint64_t dead = l2_policy_dead(p.l2);
-  uint32_t row, mi;
-  locate(p.g, i, row, mi);
-  const bool next = p.next_table != nullptr, hist = q.prev != nullptr, fin = q.st.final != 0;
-  float av[N], bv[N], yv[N], xv[N], nv[N], pv[N], ov[N], dv[N];
-  bool known[N];
-  uint32_t kb = 0, kidx = 0;
-  if constexpr (kPk) {
-    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
-    if constexpr (N == 4) {
-      known_quad(w, i, kb, kidx);
-    } else {
-      kb = (w.x >> (i & 31u)) & 1u;
-      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
-    }
-#pragma unroll
-    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
-  } else {
-    load_m<N>(p.mask, mi, known);
-  }
-  bool any_known = false, any_free = false;
-#pragma unroll
-  for (int j = 0; j < N; ++j) {
-    any_known |= known[j];
-    any_free |= !known[j];
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = pv[j] = 0.f;
-  if constexpr (kPk) {
-    if constexpr (N == 4) {
-      gather_known4<false>(p.yk, kb, kidx, yv);
-    } else {
-      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
-    }
-  } else {
-    load_f_ro<N>(p.y, i, yv);
-  }
-  if (any_free) {
-    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
-    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
-  }
-  const bool update = any_free || !next;  // somewhere in the vector x's update is not overwritten by the replace step
-  if ((update && !fin) || q.dout) load_f<N>(p.x, i, xv);
-  if (hist && update) load_head_ro<N, float>(q.prev, i, pv, dead);  // nothing reads it again
-  float rn = 0.f, ry = 0.f;
-  if (next) {
-    if constexpr (kPk) {
-      if constexpr (N == 4) {
-        gather_known4<false>(p.nk, kb, kidx, nv);
-      } else {
-        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
-      }
-    } else {
-      if (any_known) load_f_ro<N>(p.noise, i, nv);
-    }
-    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
-    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j)
-    ge_element(av[j], bv[j], yv[j], nv[j], pv[j], known[j], xv[j], ov[j], dv[j], p.combine != 0, p.cfg, q.st, fin,
-               hist, next, rn, ry);
-  if (p.out) store_f<N>(p.out, i, ov, dead);
-  if (q.dout) store_f<N>(q.dout, i, dv);  // normal policy: the next step reads it
-  store_f<N>(p.x, i, xv);
-  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
-    if (p.discard) {
-      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
-      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
-        __syncwarp();           // every lane's head loads are used
-        discard_line<H>(p.a, i, end);
-        if (p.b) discard_line<H>(p.b, i, end);
-      }
-    }
-  }
+  const uint32_t i = (walk_index(q.b.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= q.b.g.total) return;
+  GeUpdate<N> u{q};
+  boundary_vector<N, H, kPk>(q.b, i, u);
 }
 
-template <typename H>
-int ge_dispatch(const GeArgs& q, bool v4, cudaStream_t s) {
-  const uint32_t total = q.b.g.total;
-  if (q.b.kwords) {
-    if (v4) launch_kernel(boundary_ge_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_ge_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
-  } else {
-    if (v4) launch_kernel(boundary_ge_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_ge_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
-  }
-  return check_launch();
-}
+template <int N, typename H, bool kPk>
+constexpr auto ldg_kernel(const GeArgs&) { return boundary_ge_kernel<N, H, kPk>; }
 
 static int boundary_ge_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
                             const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev,
                             const lp_gradient_estimation* step, const float* next_table, const lp_dims* dims,
                             lp_stream_t stream) {
-  if (int rc = boundary_check(mo, y, noise, mask, known, x_inout, out, next_table)) return rc;
-  if (!x_inout || !step || (step->final && d_prev)) return LP_ERR_INVALID;
   GeArgs q;
-  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  bool v4;
   // the launch writes x, out and d_out while it reads d_prev: the four share no byte
-  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
-  const auto any = [&](const void* u, const void* v) { return u && v && (u == v || overlaps(u, v, bytes)); };
-  const void* bufs[4] = {x_inout, out, d_out, d_prev};
-  for (int k = 0; k < 4; ++k)
-    for (int l = 0; l < k; ++l)
-      if (any(bufs[k], bufs[l])) return LP_ERR_INVALID;
+  if (int rc = boundary_setup(q.b, v4, x_inout && step && !(step->final && d_prev), mo, y, noise, mask, known, x_inout,
+                              out, 0.f, next_table, dims, {x_inout, out, d_out, d_prev}, 0))
+    return rc;
   if (q.b.g.total == 0) return LP_OK;
-  boundary_args(q.b, mo, y, noise, mask, known, x_inout, out, 0.f, next_table);
-  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x_inout, out, d_out, d_prev});  // no state dropped
   q.st = *step;
   q.dout = d_out;
   q.prev = d_prev;
-  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
-  const bool v4 = boundary_vec4(q.b, dtype) && (!d_out || aligned16(d_out)) && (!d_prev || aligned16(d_prev));
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case LP_DTYPE_F32: return ge_dispatch<float>(q, v4, s);
-    case LP_DTYPE_BF16: return ge_dispatch<__nv_bfloat16>(q, v4, s);
-    default: return ge_dispatch<__half>(q, v4, s);
-  }
+  return launch_ldg(q, q.b, mo->dtype & ~LP_HEADS_DEAD, v4, (cudaStream_t)stream);
 }
 
 // ---- the boundary of the second wrapper call of a host-owned Heun loop ------------------------------------------
@@ -1442,146 +1104,57 @@ struct HeunArgs {
   const float* prev;    // the first call's out
 };
 
-// per element: den = combine ? b + (a-b) cfg : a ; o = known ? y : den ; d = (x - prev) / sigma ;
-// d2 = (x2 - o) / sigma_next ; x = x + ((d + d2) * 0.5) dt ; x = known ? rn n + ry y : x
-__device__ __forceinline__ void heun_element(float a, float b, float y, float nz, float v2, float pv, bool known,
-                                             float& x, float& o, bool combine, float cfg, const lp_heun& st, bool next,
-                                             float rn, float ry) {
-  const float den = combine ? __fadd_rn(b, __fmul_rn(__fsub_rn(a, b), cfg)) : a;
-  o = known ? y : den;
-  const float d = __fdiv_rn(__fsub_rn(x, pv), st.sigma);
-  const float d2 = __fdiv_rn(__fsub_rn(v2, o), st.sigma_next);
-  // torch divides by the Python scalar 2 as a multiply by 0.5: the same bits, there being no flush to zero
-  const float u = __fadd_rn(x, __fmul_rn(__fmul_rn(__fadd_rn(d, d2), 0.5f), st.dt));
-  x = next && known ? fmaf(rn, nz, ry * y) : u;  // the replace step rounds as prologue_kernel does
-}
-
-// boundary_kernel's form and operand skipping; x, x2 and the first call's out are read where x's update survives
-template <int N, typename H, bool kPk>
-__global__ void __launch_bounds__(kBlock) boundary_heun_kernel(const HeunArgs q) {
-  pdl_prologue();
-  const BoundaryArgs& p = q.b;
-  const uint32_t i = (walk_index(p.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
-  if (i >= p.g.total) return;
-  const uint64_t dead = l2_policy_dead(p.l2);
-  uint32_t row, mi;
-  locate(p.g, i, row, mi);
-  const bool next = p.next_table != nullptr;
-  float av[N], bv[N], yv[N], xv[N], nv[N], v2[N], pv[N], ov[N];
-  bool known[N];
-  uint32_t kb = 0, kidx = 0;
-  if constexpr (kPk) {
-    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.kwords) + (i >> 5));
-    if constexpr (N == 4) {
-      known_quad(w, i, kb, kidx);
-    } else {
-      kb = (w.x >> (i & 31u)) & 1u;
-      kidx = w.y + __popc(w.x & ((1u << (i & 31u)) - 1u));
-    }
-#pragma unroll
-    for (int j = 0; j < N; ++j) known[j] = ((kb >> j) & 1u) != 0;
-  } else {
-    load_m<N>(p.mask, mi, known);
-  }
-  bool any_known = false, any_free = false;
-#pragma unroll
-  for (int j = 0; j < N; ++j) {
-    any_known |= known[j];
-    any_free |= !known[j];
-  }
-#pragma unroll
-  for (int j = 0; j < N; ++j) av[j] = bv[j] = xv[j] = nv[j] = v2[j] = pv[j] = 0.f;
-  if constexpr (kPk) {
-    if constexpr (N == 4) {
-      gather_known4<false>(p.yk, kb, kidx, yv);
-    } else {
-      yv[0] = kb ? __ldg(p.yk + kidx) : 0.f;
-    }
-  } else {
-    load_f_ro<N>(p.y, i, yv);
-  }
-  if (any_free) {
-    load_head_ro<N, H>(static_cast<const H*>(p.a), i, av, dead);
-    if (p.combine) load_head_ro<N, H>(static_cast<const H*>(p.b), i, bv, dead);
-  }
-  if (any_free || !next) {  // somewhere in the vector x's update is not overwritten by the replace step
-    load_f<N>(p.x, i, xv);
+// d = (x - prev) / sigma ; d2 = (x2 - o) / sigma_next ; x = x + ((d + d2) * 0.5) dt ; x, x2 and the first call's out
+// read where x's update survives
+template <int N>
+struct HeunUpdate {
+  static constexpr bool kDiscard = true;
+  const HeunArgs& q;
+  float xv[N] = {}, v2[N] = {}, pv[N] = {};
+  __device__ __forceinline__ void load(uint32_t i, bool update, uint64_t dead) {
+    if (!update) return;
+    load_f<N>(q.b.x, i, xv);
     load_head_ro<N, float>(q.x2, i, v2, dead);    // the next predictor overwrites it unread
     load_head_ro<N, float>(q.prev, i, pv, dead);  // so does the next first call
   }
-  float rn = 0.f, ry = 0.f;
-  if (next) {
-    if constexpr (kPk) {
-      if constexpr (N == 4) {
-        gather_known4<false>(p.nk, kb, kidx, nv);
-      } else {
-        nv[0] = kb ? __ldg(p.nk + kidx) : 0.f;
-      }
-    } else {
-      if (any_known) load_f_ro<N>(p.noise, i, nv);
-    }
-    rn = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPN);
-    ry = __ldg(p.next_table + (size_t)row * LP_TABLE_STRIDE + LP_T_REPY);
+  __device__ __forceinline__ float& update(int j, float o) {
+    const float d = __fdiv_rn(__fsub_rn(xv[j], pv[j]), q.st.sigma);
+    const float d2 = __fdiv_rn(__fsub_rn(v2[j], o), q.st.sigma_next);
+    // torch divides by the Python scalar 2 as a multiply by 0.5: the same bits, there being no flush to zero
+    xv[j] = __fadd_rn(xv[j], __fmul_rn(__fmul_rn(__fadd_rn(d, d2), 0.5f), q.st.dt));
+    return xv[j];
   }
-#pragma unroll
-  for (int j = 0; j < N; ++j)
-    heun_element(av[j], bv[j], yv[j], nv[j], v2[j], pv[j], known[j], xv[j], ov[j], p.combine != 0, p.cfg, q.st, next,
-                 rn, ry);
-  if (p.out) store_f<N>(p.out, i, ov, dead);
-  store_f<N>(p.x, i, xv);  // normal policy: the next network call reads x first
-  if constexpr (32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
-    if (p.discard) {
-      const uint32_t end = i - (threadIdx.x & 31u) * N + 32u * N;  // end of this warp's span
-      if (end <= p.g.total) {   // warp-uniform: a partial last warp keeps its lines
-        __syncwarp();           // every lane's head loads are used
-        discard_line<H>(p.a, i, end);
-        if (p.b) discard_line<H>(p.b, i, end);
-      }
-    }
+  __device__ __forceinline__ void store(uint32_t i) {
+    store_f<N>(q.b.x, i, xv);  // normal policy: the next network call reads x first
   }
+};
+
+template <int N, typename H, bool kPk>
+__global__ void __launch_bounds__(kBlock) boundary_heun_kernel(const HeunArgs q) {
+  pdl_prologue();
+  const uint32_t i = (walk_index(q.b.l2, blockIdx.x, gridDim.x) * kBlock + threadIdx.x) * N;
+  if (i >= q.b.g.total) return;
+  HeunUpdate<N> u{q};
+  boundary_vector<N, H, kPk>(q.b, i, u);
 }
 
-template <typename H>
-int heun_dispatch(const HeunArgs& q, bool v4, cudaStream_t s) {
-  const uint32_t total = q.b.g.total;
-  if (q.b.kwords) {
-    if (v4) launch_kernel(boundary_heun_kernel<4, H, true>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_heun_kernel<1, H, true>, dim3(blocks_for(total)), s, q);
-  } else {
-    if (v4) launch_kernel(boundary_heun_kernel<4, H, false>, dim3(blocks_for(total / 4)), s, q);
-    else launch_kernel(boundary_heun_kernel<1, H, false>, dim3(blocks_for(total)), s, q);
-  }
-  return check_launch();
-}
+template <int N, typename H, bool kPk>
+constexpr auto ldg_kernel(const HeunArgs&) { return boundary_heun_kernel<N, H, kPk>; }
 
 static int boundary_heun_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
                               const lp_known* known, float* x, const float* x2, const float* out_prev, float* out,
                               const lp_heun* step, const float* next_table, const lp_dims* dims, lp_stream_t stream) {
-  if (int rc = boundary_check(mo, y, noise, mask, known, x, out, next_table)) return rc;
-  if (!step || !x || !x2 || !out_prev) return LP_ERR_INVALID;
   HeunArgs q;
-  if (int rc = make_geometry(dims, q.b.g)) return rc;
+  bool v4;
   // the launch writes x and out while it reads x2 and out_prev: the four share no byte
-  const size_t bytes = (size_t)q.b.g.total * sizeof(float);
-  const auto any = [&](const void* u, const void* v) { return u && v && (u == v || overlaps(u, v, bytes)); };
-  const void* bufs[4] = {x, x2, out_prev, out};
-  for (int k = 0; k < 4; ++k)
-    for (int l = 0; l < k; ++l)
-      if (any(bufs[k], bufs[l])) return LP_ERR_INVALID;
+  if (int rc = boundary_setup(q.b, v4, step && x && x2 && out_prev, mo, y, noise, mask, known, x, out, 0.f, next_table,
+                              dims, {x, x2, out_prev, out}, 0))
+    return rc;
   if (q.b.g.total == 0) return LP_OK;
-  boundary_args(q.b, mo, y, noise, mask, known, x, out, 0.f, next_table);
-  q.b.discard = heads_discard(mo, q.b.b, q.b.g.total, {x, x2, out_prev, out});  // a dropped line holds no state
   q.st = *step;
   q.x2 = x2;
   q.prev = out_prev;
-  const int dtype = mo->dtype & ~LP_HEADS_DEAD;
-  const bool v4 = boundary_vec4(q.b, dtype) && aligned16(x2) && aligned16(out_prev);
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case LP_DTYPE_F32: return heun_dispatch<float>(q, v4, s);
-    case LP_DTYPE_BF16: return heun_dispatch<__nv_bfloat16>(q, v4, s);
-    default: return heun_dispatch<__half>(q, v4, s);
-  }
+  return launch_ldg(q, q.b, mo->dtype & ~LP_HEADS_DEAD, v4, (cudaStream_t)stream);
 }
 
 // ---- un-fused OU advance (advance_time_overdamped, lanpaint.py:232-254) --------
