@@ -35,8 +35,9 @@ extern "C" {
  * rejected with LP_ERR_INVALID, so no earlier caller can have set it); 2 = lp_multistep and
  * lp_boundary_multistep (a new entry point: nothing an earlier caller binds changes).  Later entry points
  * (lp_midpoint and lp_boundary_midpoint, lp_deis and lp_boundary_deis, lp_gradient_estimation and
- * lp_boundary_gradient_estimation, lp_heun and lp_boundary_heun) leave LP_ABI_MINOR at 2: a caller detects one by
- * its symbol, which is how lanpaint_b200._native binds every entry point (by name). */
+ * lp_boundary_gradient_estimation, lp_heun and lp_boundary_heun, the row-bounded lp_boundary_*_rows forms) leave
+ * LP_ABI_MINOR at 2: a caller detects one by its symbol, which is how lanpaint_b200._native binds every entry point
+ * (by name). */
 #define LP_ABI_MINOR 2
 #define LP_TABLE_STRIDE 32 /* floats per table row (one 128-byte line), layout below */
 
@@ -348,6 +349,17 @@ int lp_boundary_known(const lp_heads* model_out, const float* y, const float* no
                       const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
                       const lp_dims* dims, lp_stream_t stream);
 
+/* Row-bounded `out`.  Each lp_boundary_*_rows entry point is the entry point of the same name without the suffix,
+ * except that `out` is stored only for the first out_rows rows (elements < out_rows * per_row): out then needs room
+ * for min(out_rows, n_rows) rows only, and no byte past them is written.  out_rows >= n_rows is the entry point itself,
+ * out_rows == 0 stores no out, like out == NULL, and out_rows < 0 is LP_ERR_INVALID.  Every other store, x included,
+ * and which heads' lines are dropped (LP_HEADS_DEAD) are unchanged.  A host whose denoised latent is read only by a
+ * preview of the first request passes 1.  (lp_boundary_multistep and lp_boundary_heun have no such form: the host
+ * reads their out back whole in a later launch.) */
+int lp_boundary_known_rows(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                           const lp_known* known, float* x_inout, float* out, int64_t out_rows, float euler_coef,
+                           const float* next_table, const lp_dims* dims, lp_stream_t stream);
+
 /* One outer step of k-diffusion's sample_euler_ancestral, as the host precomputes it (get_ancestral_step in Python
  * doubles, then one rounding to fp32 per field). */
 typedef struct lp_ancestral {
@@ -373,6 +385,11 @@ typedef struct lp_ancestral {
 int lp_boundary_ancestral(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                           const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
                           const lp_rng* rng, const float* next_table, const lp_dims* dims, lp_stream_t stream);
+/* lp_boundary_ancestral with a row-bounded out (see lp_boundary_known_rows). */
+int lp_boundary_ancestral_rows(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                               const lp_known* known, float* x_inout, float* out, int64_t out_rows,
+                               const lp_ancestral* step, const lp_rng* rng, const float* next_table,
+                               const lp_dims* dims, lp_stream_t stream);
 
 /* One outer step of k-diffusion's sample_dpmpp_2m (DPM-Solver++(2M)), with t = -log(sigma) and h = t_next - t.  The
  * host evaluates these with the sampler's own torch expressions on the schedule, on the device the sampler runs on,
@@ -431,6 +448,11 @@ typedef struct lp_midpoint {
 int lp_boundary_midpoint(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                          const lp_known* known, const float* x_in, const float* x_base, float* x_out, float* out,
                          const lp_midpoint* step, const float* next_table, const lp_dims* dims, lp_stream_t stream);
+/* lp_boundary_midpoint with a row-bounded out (see lp_boundary_known_rows). */
+int lp_boundary_midpoint_rows(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                              const lp_known* known, const float* x_in, const float* x_base, float* x_out, float* out,
+                              int64_t out_rows, const lp_midpoint* step, const float* next_table, const lp_dims* dims,
+                              lp_stream_t stream);
 
 /* One outer step of ComfyUI's sample_deis (DEIS, max_order 3, 'tab' mode): x = x + c_cur*d [+ c_prev1*d_{i-1}
  * [+ c_prev2*d_{i-2}]] with d = (x - out) / sigma.  The host takes the coefficients from the sampler's own
@@ -464,6 +486,11 @@ int lp_boundary_deis(const lp_heads* model_out, const float* y, const float* noi
                      const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev1,
                      const float* d_prev2, const lp_deis* step, const float* next_table, const lp_dims* dims,
                      lp_stream_t stream);
+/* lp_boundary_deis with a row-bounded out (see lp_boundary_known_rows). */
+int lp_boundary_deis_rows(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                          const lp_known* known, float* x_inout, float* out, int64_t out_rows, float* d_out,
+                          const float* d_prev1, const float* d_prev2, const lp_deis* step, const float* next_table,
+                          const lp_dims* dims, lp_stream_t stream);
 
 /* One outer step of ComfyUI's sample_gradient_estimation (ge_gamma, no cfg_pp): the Euler step x = x + d*dt and,
  * from the second step on, the gradient-estimation correction x = x + (gm1*(d - d_prev))*dt, with d = (x - out) / sigma;
@@ -496,6 +523,12 @@ int lp_boundary_gradient_estimation(const lp_heads* model_out, const float* y, c
                                     const lp_known* known, float* x_inout, float* out, float* d_out,
                                     const float* d_prev, const lp_gradient_estimation* step, const float* next_table,
                                     const lp_dims* dims, lp_stream_t stream);
+/* lp_boundary_gradient_estimation with a row-bounded out (see lp_boundary_known_rows). */
+int lp_boundary_gradient_estimation_rows(const lp_heads* model_out, const float* y, const float* noise,
+                                         const uint8_t* mask, const lp_known* known, float* x_inout, float* out,
+                                         int64_t out_rows, float* d_out, const float* d_prev,
+                                         const lp_gradient_estimation* step, const float* next_table,
+                                         const lp_dims* dims, lp_stream_t stream);
 
 /* The corrector of k-diffusion's sample_heun (no churn, so sigma_hat = sigma_i): x = x + ((d + d_2) / 2) * dt with
  * d = (x - denoised) / sigma_i from the step's first wrapper call and d_2 = (x_2 - denoised_2) / sigma_next from its

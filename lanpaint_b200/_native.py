@@ -26,7 +26,8 @@ SYMBOLS = (
     "lp_abi_version", "lp_status_string", "lp_last_cuda_error", "lp_set_option", "lp_selftest_index_math", "lp_selftest_box_muller", "lp_selftest_normal_fast", "lp_build_coef_table", "lp_build_coef_table_dt",
     "lp_torch_randn_geometry", "lp_pack_mask_f32", "lp_prologue_f32", "lp_substep", "lp_substep_f32", "lp_substep_cfg_f32", "lp_advance_f32",
     "lp_boundary", "lp_boundary_ancestral", "lp_boundary_multistep", "lp_boundary_midpoint", "lp_boundary_deis", "lp_boundary_gradient_estimation",
-    "lp_boundary_heun", "lp_synth_denoiser", "lp_known_words", "lp_pack_known", "lp_substep_known", "lp_boundary_known",
+    "lp_boundary_heun", "lp_boundary_known_rows", "lp_boundary_ancestral_rows", "lp_boundary_midpoint_rows",
+    "lp_boundary_deis_rows", "lp_boundary_gradient_estimation_rows", "lp_synth_denoiser", "lp_known_words", "lp_pack_known", "lp_substep_known", "lp_boundary_known",
     "lp_epilogue_f32", "lp_epilogue_euler_f32", "lp_step_boundary_f32", "lp_epilogue_cfg_f32", "lp_stop_stats_f32", "lp_fill_normal_f32", "lp_synth_denoiser_f32", "lp_l2_persist_capacity", "lp_l2_persist_set", "lp_l2_persist_clear", "lp_l2_flush", "lp_torch_cpu_randn_f32",
 )
 
@@ -165,6 +166,13 @@ def load() -> C.CDLL:
     lib.lp_boundary_heun.restype = i32
     lib.lp_boundary_heun.argtypes = [C.POINTER(Heads), p, p, p, C.POINTER(Known), p, p, p, p, C.POINTER(Heun), p,
                                      C.POINTER(Dims), p]
+    # the row-bounded forms: `out_rows` (int64) right after `out`
+    for name in ("lp_boundary_known", "lp_boundary_ancestral", "lp_boundary_midpoint", "lp_boundary_deis",
+                 "lp_boundary_gradient_estimation"):
+        f, g = getattr(lib, name), getattr(lib, name + "_rows")
+        out = {"lp_boundary_midpoint": 8}.get(name, 6)   # position of `out`
+        g.restype = i32
+        g.argtypes = f.argtypes[:out + 1] + [i64] + f.argtypes[out + 1:]
     lib.lp_synth_denoiser.restype = i32
     lib.lp_synth_denoiser.argtypes = [p, p, p, i32, i64, p, p]
     lib.lp_substep_f32.restype = i32

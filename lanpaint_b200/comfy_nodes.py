@@ -671,23 +671,29 @@ class KSAMPLER(comfy.samplers.KSAMPLER):
             # keeps it live -- right for a real network, where a step takes long enough to watch.  When the eager
             # job of this configuration took only a few (< 50) milliseconds nobody can watch anything: the whole job runs
             # as ONE graph, each outer step keeps its denoised latent, and the callbacks run in order right after.
-            dev_ms = None      # device time of this configuration's previous job (the very first one of a process
-            if entry.eager_events is not None:   # also pays CUDA's lazy module loading and is re-measured)
-                dev_ms = entry.eager_events[0].elapsed_time(entry.eager_events[1])
+            dev_ms = None      # device time of this configuration's previous job
+            if entry.eager_events is not None:
+                dev_ms = entry.eager_events[0].elapsed_time(entry.eager_events[1]) * entry.eager_scale
             deferred = (opts.get("deferred_callbacks", True) and dev_ms is not None
                         and dev_ms <= float(opts.get("deferred_max_ms", 50.0))
                         and job.per_step_bytes() <= int(opts.get("deferred_max_bytes", 4 << 30)))
             mode = "job" if deferred else "steps"
+        observe = _deferred_outputs(callback, opts)
         timing = None
         if entry is not None:
             timing = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
             timing[0].record()
         try:
             out = job.run(latent_image, model_k.noise, pm, x_init=x_init, callback=callback, mode=mode,
-                          warm=after <= 0)
+                          warm=after <= 0, observe=observe)
             if timing is not None and job.captures == captures:   # a run that captured graphs also timed the capture
                 timing[1].record()
-                entry.eager_events = timing
+                entry.eager_events, entry.eager_scale = timing, 1.0
+                n = len(job.sched.steps)
+                if mode == "eager" and n > 1:
+                    # the first outer step of the first job of a process also loads every kernel the job launches
+                    # (CUDA's lazy module loading), which can take as long as the job: time the other steps
+                    entry.eager_events, entry.eager_scale = (job.first_step_end, timing[1]), n / (n - 1)
         except Exception as e:
             if mode == "eager":
                 raise
@@ -854,6 +860,42 @@ def _restates(fn, sampler: str) -> bool:
 # =============================================================================================
 # engines (and their CUDA graphs) kept across sample() calls
 # =============================================================================================
+# ComfyUI's own previewers (latent_preview.py): each decodes the first request's latent, x0[:1], and nothing else
+_STOCK_PREVIEWERS = ("Latent2RGBPreviewer", "TAESDPreviewerImpl")
+
+
+def _deferred_outputs(callback, opts) -> str:
+    """What of each outer step's denoised latent a deferred fused job keeps for `callback` (GraphedJob.run's observe).
+
+    ComfyUI's stock callback, the closure `latent_preview.prepare_callback` returns, stores x0 into its output dict
+    (each step overwriting the last), hands it to the previewer, if one is configured, and advances the progress bar.
+    So before the last step it reads only what the previewer decodes, the first request's latent: "final" without a
+    previewer, "preview" with one of ComfyUI's own.  Any other callback -- a user's, one from a patched or replaced
+    prepare_callback, one whose previewer is not ComfyUI's -- gets "full", every step's whole latent, as does the model
+    option {"lanpaint_b200": {"deferred_outputs": "full"}}.  The stock closure is told by its code object: one of the
+    functions compiled into the current prepare_callback, itself ComfyUI's (minicomfy's in tests) by name and module."""
+    setting = opts.get("deferred_outputs", "auto")
+    if setting not in ("auto", "full"):
+        raise ValueError(f"lanpaint_b200 option deferred_outputs: 'auto' or 'full', not {setting!r}")
+    prepare = getattr(latent_preview, "prepare_callback", None)
+    code = getattr(callback, "__code__", None)
+    if setting == "full" or code is None or not (getattr(prepare, "__qualname__", "") == "prepare_callback" and
+                                                 getattr(prepare, "__module__", "") in ("latent_preview", "minicomfy")):
+        return "full"
+    if code not in prepare.__code__.co_consts:
+        return "full"
+    cells = dict(zip(code.co_freevars, callback.__closure__ or ()))
+    if not set(cells) <= {"x0_output_dict", "previewer", "pbar", "preview_format"}:
+        return "full"
+    previewer = cells["previewer"].cell_contents if "previewer" in cells else None
+    if not previewer:
+        return "final"
+    kind = type(previewer)
+    if kind.__name__ in _STOCK_PREVIEWERS and kind.__module__ in ("latent_preview", "minicomfy"):
+        return "preview"
+    return "full"
+
+
 def _graphs_enabled(opts) -> bool:
     import os
     if os.environ.get("LANPAINT_B200_GRAPH", "1") == "0":
@@ -894,7 +936,7 @@ def _cond_fingerprint(c, depth: int = 0):
 
 class _EngineEntry:
     __slots__ = ("engine", "job", "runs", "graph_failed", "last_mode", "weights", "keep", "pinned", "eager_events",
-                 "trace", "sampler_job", "sg_retries")
+                 "eager_scale", "trace", "sampler_job", "sg_retries")
 
     def __init__(self):
         self.engine = self.job = None
@@ -903,6 +945,7 @@ class _EngineEntry:
         self.sg_retries = 0
         self.pinned = []
         self.eager_events = None   # CUDA events around the previous job: how long this configuration takes
+        self.eager_scale = 1.0     # ... times this (the events span only part of it)
         self.runs = 0
         self.graph_failed = False
         self.last_mode = None

@@ -57,6 +57,7 @@ struct BoundaryArgs {
   const float* nk;         // noise at known elements
   float* x;        // NULL: no Euler update
   float* out;      // NULL: nobody reads the denoised latent
+  uint32_t out_end;  // out is stored for elements < out_end only: its first out_rows rows
   const float* next_table;  // NULL: no replace step of the next outer step
   float cfg, coef;
   int combine;
@@ -158,7 +159,7 @@ __device__ __forceinline__ void boundary_vector(const BoundaryArgs& p, uint32_t 
     float& x = u.update(j, ov[j]);
     if (next) x = k ? fmaf(rn, nv[j], ry * yv[j]) : x;  // rounds as prologue_kernel does
   }
-  if (p.out) store_f<N>(p.out, i, ov, dead);
+  if (p.out && i < p.out_end) store_f<N>(p.out, i, ov, dead);  // a vector lies in one row
   u.store(i);
   if constexpr (U::kDiscard && 32 * N * sizeof(H) >= 128) {  // a warp's span holds whole lines
     if (p.discard) {
@@ -289,7 +290,7 @@ __global__ void __launch_bounds__(kBlock, 2) boundary_tma_kernel(const BoundaryA
         for (int j = 0; j < 4; ++j)
           boundary_element(av[j], bv[j], y[j], nz[j], known[j], x[j], o[j], kCombine, p.cfg, p.coef, true, kNext, rn, ry);
         const uint32_t i = e0 + 4 * v;
-        if (p.out) st_f4(p.out + i, make_float4(o[0], o[1], o[2], o[3]), dead);
+        if (p.out && i < p.out_end) st_f4(p.out + i, make_float4(o[0], o[1], o[2], o[3]), dead);
         *reinterpret_cast<float4*>(p.x + i) = make_float4(x[0], x[1], x[2], x[3]);
       }
     }
@@ -365,16 +366,18 @@ static int boundary_check(const lp_heads* mo, const float* y, const float* noise
   return LP_OK;
 }
 
-// Whether two of `bufs` -- fp32 buffers of `bytes` each, NULL entries absent -- share a byte.  A pair from the first
-// `k` is exempt: the launch lets those alias, and with `whole` they may be one buffer but must not overlap in part
-// (each element is read and written by one thread).
-static bool aliased(std::initializer_list<const void*> bufs, size_t bytes, size_t k, bool whole) {
+// Whether two of `bufs` -- fp32 buffers of `bytes` each but `out`, which spans out_bytes, NULL entries absent --
+// share a byte.  A pair from the first `k` is exempt: the launch lets those alias, and with `whole` they may be one
+// buffer but must not overlap in part (each element is read and written by one thread).
+static bool aliased(std::initializer_list<const void*> bufs, size_t bytes, const void* out, size_t out_bytes, size_t k,
+                    bool whole) {
   const void* const* v = bufs.begin();
   for (size_t m = 1; m < bufs.size(); ++m)
     for (size_t l = 0; l < m; ++l) {
       if (!v[m] || !v[l]) continue;
       const uintptr_t u = reinterpret_cast<uintptr_t>(v[m]), w = reinterpret_cast<uintptr_t>(v[l]);
-      const bool shared = u == w || (u < w + bytes && w < u + bytes);
+      const size_t un = v[m] == out ? out_bytes : bytes, wn = v[l] == out ? out_bytes : bytes;
+      const bool shared = u == w || (u < w + wn && w < u + un);
       if (m < k ? whole && shared && u != w : shared) return true;
     }
   return false;
@@ -382,23 +385,28 @@ static bool aliased(std::initializer_list<const void*> bufs, size_t bytes, size_
 
 // The setup every boundary entry point shares, before any CUDA call: the checks (the sampler's own are `valid`), the
 // geometry, the aliasing rule on `states` (every fp32 buffer the launch reads or writes besides y and the noise, see
-// aliased), the operands, whether the heads' lines may be dropped and whether the launch runs 4-wide.  An empty
-// launch returns LP_OK with p.g.total == 0.
+// aliased), the operands, whether the heads' lines may be dropped and whether the launch runs 4-wide.  `out` holds
+// its first out_rows rows (out_rows < 0: every row).  An empty launch returns LP_OK with p.g.total == 0.
 static int boundary_setup(BoundaryArgs& p, bool& v4, bool valid, const lp_heads* mo, const float* y, const float* noise,
-                          const uint8_t* mask, const lp_known* known, float* x, float* out, float euler_coef,
-                          const float* next_table, const lp_dims* dims, std::initializer_list<const void*> states,
-                          size_t k, bool whole = false) {
+                          const uint8_t* mask, const lp_known* known, float* x, float* out, int64_t out_rows,
+                          float euler_coef, const float* next_table, const lp_dims* dims,
+                          std::initializer_list<const void*> states, size_t k, bool whole = false) {
   v4 = false;
   if (int rc = boundary_check(mo, y, noise, mask, known, x, out, next_table)) return rc;
   if (!valid) return LP_ERR_INVALID;
   if (int rc = make_geometry(dims, p.g)) return rc;
-  if (aliased(states, (size_t)p.g.total * sizeof(float), k, whole)) return LP_ERR_INVALID;
+  const uint32_t out_end = out_rows < 0 || (uint64_t)out_rows >= p.g.n_rows
+                               ? p.g.total : (uint32_t)out_rows * p.g.per_row.d;
+  const size_t bytes = (size_t)p.g.total * sizeof(float), out_bytes = (size_t)out_end * sizeof(float);
+  if (aliased(states, bytes, out, out_bytes, k, whole)) return LP_ERR_INVALID;
   if (p.g.total == 0) return LP_OK;
-  p.a = mo->a; p.b = mo->combine ? mo->b : nullptr; p.y = y; p.noise = noise; p.mask = mask; p.x = x; p.out = out;
+  p.a = mo->a; p.b = mo->combine ? mo->b : nullptr; p.y = y; p.noise = noise; p.mask = mask; p.x = x;
+  p.out = out_end ? out : nullptr;  // no row: the launch stores no out, as with out == NULL
+  p.out_end = out_end;
   p.kwords = known ? known->words : nullptr; p.yk = known ? known->y : nullptr; p.nk = known ? known->noise : nullptr;
   p.next_table = next_table; p.cfg = mo->cfg; p.coef = euler_coef; p.combine = mo->combine != 0;
   p.l2 = l2_handoff(p.g.total);
-  p.discard = heads_discard(mo, p.b, p.g.total, states);  // a dropped line holds no state
+  p.discard = heads_discard(mo, p.b, p.g.total, states, out, out_bytes);  // a dropped line holds no state
   const int dtype = mo->dtype & ~LP_HEADS_DEAD;
   v4 = geometry_vec4(p.g, p.mask) && head_aligned(p.a, dtype) && (!p.b || head_aligned(p.b, dtype)) &&
        aligned16(p.y) && (!p.noise || aligned16(p.noise));
@@ -407,12 +415,12 @@ static int boundary_setup(BoundaryArgs& p, bool& v4, bool valid, const lp_heads*
 }
 
 static int boundary_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
-                         const lp_known* known, float* x_inout, float* out, float euler_coef, const float* next_table,
-                         const lp_dims* dims, lp_stream_t stream) {
+                         const lp_known* known, float* x_inout, float* out, int64_t out_rows, float euler_coef,
+                         const float* next_table, const lp_dims* dims, lp_stream_t stream) {
   BoundaryArgs p;
   bool v4;
-  if (int rc = boundary_setup(p, v4, true, mo, y, noise, mask, known, x_inout, out, euler_coef, next_table, dims,
-                              {x_inout, out}, 2))
+  if (int rc = boundary_setup(p, v4, true, mo, y, noise, mask, known, x_inout, out, out_rows, euler_coef, next_table,
+                              dims, {x_inout, out}, 2))
     return rc;
   if (p.g.total == 0) return LP_OK;
   cudaStream_t s = (cudaStream_t)stream;
@@ -702,7 +710,7 @@ __global__ void __launch_bounds__(1024 / 4 + 32, 2)
     for (int e = 0; e < 4; ++e)
       ancestral_element(a[e], b[e], y[e], nz[e], ((kb >> e) & 1u) != 0, x[e], o[e], kCombine, p.cfg, q.st, true, xi[e],
                         kNext, rn, ry);
-    if (p.out) st_f4(p.out + i, make_float4(o[0], o[1], o[2], o[3]), l2_policy_dead(p.l2));
+    if (p.out && i < p.out_end) st_f4(p.out + i, make_float4(o[0], o[1], o[2], o[3]), l2_policy_dead(p.l2));
     *reinterpret_cast<float4*>(p.x + i) = make_float4(x[0], x[1], x[2], x[3]);
   };
   uint32_t it = 0;
@@ -802,7 +810,8 @@ int ancestral_dispatch(AncestralArgs& q, int mode, bool v4, cudaStream_t s) {
 }
 
 static int boundary_ancestral_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
-                                   const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
+                                   const lp_known* known, float* x_inout, float* out, int64_t out_rows,
+                                   const lp_ancestral* step,
                                    const lp_rng* rng, const float* next_table, const lp_dims* dims,
                                    lp_stream_t stream) {
   const int mode = rng ? rng->mode : kRngNone;
@@ -811,7 +820,7 @@ static int boundary_ancestral_impl(const lp_heads* mo, const float* y, const flo
                      (mode != LP_RNG_TAPE || rng->tape0);
   AncestralArgs q;
   bool v4;
-  if (int rc = boundary_setup(q.b, v4, valid, mo, y, noise, mask, known, x_inout, out, 0.f, next_table, dims,
+  if (int rc = boundary_setup(q.b, v4, valid, mo, y, noise, mask, known, x_inout, out, out_rows, 0.f, next_table, dims,
                               {x_inout, out}, 2))
     return rc;
   if (q.b.g.total == 0) return LP_OK;
@@ -876,7 +885,7 @@ static int boundary_multistep_impl(const lp_heads* mo, const float* y, const flo
   MultistepArgs q;
   bool v4;
   // the launch writes x and out while it reads old_out
-  if (int rc = boundary_setup(q.b, v4, x_inout && step, mo, y, noise, mask, known, x_inout, out, 0.f, next_table, dims,
+  if (int rc = boundary_setup(q.b, v4, x_inout && step, mo, y, noise, mask, known, x_inout, out, -1, 0.f, next_table, dims,
                               {x_inout, out, old_out}, 2))
     return rc;
   if (q.b.g.total == 0) return LP_OK;
@@ -937,14 +946,14 @@ constexpr auto ldg_kernel(const MidpointArgs&) { return boundary_midpoint_kernel
 
 static int boundary_midpoint_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
                                   const lp_known* known, const float* x_in, const float* x_base, float* x_out,
-                                  float* out, const lp_midpoint* step, const float* next_table, const lp_dims* dims,
+                                  float* out, int64_t out_rows, const lp_midpoint* step, const float* next_table, const lp_dims* dims,
                                   lp_stream_t stream) {
   MidpointArgs q;
   bool v4;
   // one thread reads and writes each element: the three states are each one buffer or disjoint, and out, which the
   // launch writes, shares no byte with any of them
-  if (int rc = boundary_setup(q.b, v4, step && x_in && x_base && x_out, mo, y, noise, mask, known, x_out, out, 0.f,
-                              next_table, dims, {x_in, x_base, x_out, out}, 3, true))
+  if (int rc = boundary_setup(q.b, v4, step && x_in && x_base && x_out, mo, y, noise, mask, known, x_out, out,
+                              out_rows, 0.f, next_table, dims, {x_in, x_base, x_out, out}, 3, true))
     return rc;
   if (q.b.g.total == 0) return LP_OK;
   q.st = *step;
@@ -1006,7 +1015,7 @@ template <int N, typename H, bool kPk>
 constexpr auto ldg_kernel(const DeisArgs&) { return boundary_deis_kernel<N, H, kPk>; }
 
 static int boundary_deis_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
-                              const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev1,
+                              const lp_known* known, float* x_inout, float* out, int64_t out_rows, float* d_out, const float* d_prev1,
                               const float* d_prev2, const lp_deis* step, const float* next_table, const lp_dims* dims,
                               lp_stream_t stream) {
   DeisArgs q;
@@ -1014,7 +1023,7 @@ static int boundary_deis_impl(const lp_heads* mo, const float* y, const float* n
   // the launch writes x, out and d_out while it reads the history: the three histories share no byte with each other
   // or with x and out
   if (int rc = boundary_setup(q.b, v4, x_inout && step && (d_prev1 || !d_prev2), mo, y, noise, mask, known, x_inout,
-                              out, 0.f, next_table, dims, {x_inout, out, d_out, d_prev1, d_prev2}, 2))
+                              out, out_rows, 0.f, next_table, dims, {x_inout, out, d_out, d_prev1, d_prev2}, 2))
     return rc;
   if (q.b.g.total == 0) return LP_OK;
   q.st = *step;
@@ -1076,14 +1085,14 @@ template <int N, typename H, bool kPk>
 constexpr auto ldg_kernel(const GeArgs&) { return boundary_ge_kernel<N, H, kPk>; }
 
 static int boundary_ge_impl(const lp_heads* mo, const float* y, const float* noise, const uint8_t* mask,
-                            const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev,
+                            const lp_known* known, float* x_inout, float* out, int64_t out_rows, float* d_out, const float* d_prev,
                             const lp_gradient_estimation* step, const float* next_table, const lp_dims* dims,
                             lp_stream_t stream) {
   GeArgs q;
   bool v4;
   // the launch writes x, out and d_out while it reads d_prev: the four share no byte
   if (int rc = boundary_setup(q.b, v4, x_inout && step && !(step->final && d_prev), mo, y, noise, mask, known, x_inout,
-                              out, 0.f, next_table, dims, {x_inout, out, d_out, d_prev}, 0))
+                              out, out_rows, 0.f, next_table, dims, {x_inout, out, d_out, d_prev}, 0))
     return rc;
   if (q.b.g.total == 0) return LP_OK;
   q.st = *step;
@@ -1147,7 +1156,7 @@ static int boundary_heun_impl(const lp_heads* mo, const float* y, const float* n
   HeunArgs q;
   bool v4;
   // the launch writes x and out while it reads x2 and out_prev: the four share no byte
-  if (int rc = boundary_setup(q.b, v4, step && x && x2 && out_prev, mo, y, noise, mask, known, x, out, 0.f, next_table,
+  if (int rc = boundary_setup(q.b, v4, step && x && x2 && out_prev, mo, y, noise, mask, known, x, out, -1, 0.f, next_table,
                               dims, {x, x2, out_prev, out}, 0))
     return rc;
   if (q.b.g.total == 0) return LP_OK;
@@ -1313,21 +1322,39 @@ extern "C" int lp_prologue_f32(const float* x, const float* y, const float* nois
 extern "C" int lp_boundary(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                            float* x_inout, float* out, float euler_coef, const float* next_table, const lp_dims* dims,
                            lp_stream_t stream) {
-  return boundary_impl(model_out, y, noise, mask, nullptr, x_inout, out, euler_coef, next_table, dims, stream);
+  return boundary_impl(model_out, y, noise, mask, nullptr, x_inout, out, -1, euler_coef, next_table, dims, stream);
 }
 
 extern "C" int lp_boundary_known(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                                  const lp_known* known, float* x_inout, float* out, float euler_coef,
                                  const float* next_table, const lp_dims* dims, lp_stream_t stream) {
   if (!known) return LP_ERR_INVALID;
-  return boundary_impl(model_out, y, noise, mask, known, x_inout, out, euler_coef, next_table, dims, stream);
+  return boundary_impl(model_out, y, noise, mask, known, x_inout, out, -1, euler_coef, next_table, dims, stream);
+}
+
+extern "C" int lp_boundary_known_rows(const lp_heads* model_out, const float* y, const float* noise,
+                                      const uint8_t* mask, const lp_known* known, float* x_inout, float* out,
+                                      int64_t out_rows, float euler_coef, const float* next_table, const lp_dims* dims,
+                                      lp_stream_t stream) {
+  if (!known || out_rows < 0) return LP_ERR_INVALID;
+  return boundary_impl(model_out, y, noise, mask, known, x_inout, out, out_rows, euler_coef, next_table, dims, stream);
 }
 
 extern "C" int lp_boundary_ancestral(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                                      const lp_known* known, float* x_inout, float* out, const lp_ancestral* step,
                                      const lp_rng* rng, const float* next_table, const lp_dims* dims,
                                      lp_stream_t stream) {
-  return boundary_ancestral_impl(model_out, y, noise, mask, known, x_inout, out, step, rng, next_table, dims, stream);
+  return boundary_ancestral_impl(model_out, y, noise, mask, known, x_inout, out, -1, step, rng, next_table, dims,
+                                 stream);
+}
+
+extern "C" int lp_boundary_ancestral_rows(const lp_heads* model_out, const float* y, const float* noise,
+                                          const uint8_t* mask, const lp_known* known, float* x_inout, float* out,
+                                          int64_t out_rows, const lp_ancestral* step, const lp_rng* rng,
+                                          const float* next_table, const lp_dims* dims, lp_stream_t stream) {
+  if (out_rows < 0) return LP_ERR_INVALID;
+  return boundary_ancestral_impl(model_out, y, noise, mask, known, x_inout, out, out_rows, step, rng, next_table, dims,
+                                 stream);
 }
 
 extern "C" int lp_boundary_multistep(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
@@ -1342,24 +1369,53 @@ extern "C" int lp_boundary_midpoint(const lp_heads* model_out, const float* y, c
                                     const lp_known* known, const float* x_in, const float* x_base, float* x_out,
                                     float* out, const lp_midpoint* step, const float* next_table, const lp_dims* dims,
                                     lp_stream_t stream) {
-  return boundary_midpoint_impl(model_out, y, noise, mask, known, x_in, x_base, x_out, out, step, next_table, dims,
+  return boundary_midpoint_impl(model_out, y, noise, mask, known, x_in, x_base, x_out, out, -1, step, next_table, dims,
                                 stream);
+}
+
+extern "C" int lp_boundary_midpoint_rows(const lp_heads* model_out, const float* y, const float* noise,
+                                         const uint8_t* mask, const lp_known* known, const float* x_in,
+                                         const float* x_base, float* x_out, float* out, int64_t out_rows,
+                                         const lp_midpoint* step, const float* next_table, const lp_dims* dims,
+                                         lp_stream_t stream) {
+  if (out_rows < 0) return LP_ERR_INVALID;
+  return boundary_midpoint_impl(model_out, y, noise, mask, known, x_in, x_base, x_out, out, out_rows, step, next_table,
+                                dims, stream);
 }
 
 extern "C" int lp_boundary_deis(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
                                 const lp_known* known, float* x_inout, float* out, float* d_out, const float* d_prev1,
                                 const float* d_prev2, const lp_deis* step, const float* next_table, const lp_dims* dims,
                                 lp_stream_t stream) {
-  return boundary_deis_impl(model_out, y, noise, mask, known, x_inout, out, d_out, d_prev1, d_prev2, step, next_table,
-                            dims, stream);
+  return boundary_deis_impl(model_out, y, noise, mask, known, x_inout, out, -1, d_out, d_prev1, d_prev2, step,
+                            next_table, dims, stream);
+}
+
+extern "C" int lp_boundary_deis_rows(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
+                                     const lp_known* known, float* x_inout, float* out, int64_t out_rows, float* d_out,
+                                     const float* d_prev1, const float* d_prev2, const lp_deis* step,
+                                     const float* next_table, const lp_dims* dims, lp_stream_t stream) {
+  if (out_rows < 0) return LP_ERR_INVALID;
+  return boundary_deis_impl(model_out, y, noise, mask, known, x_inout, out, out_rows, d_out, d_prev1, d_prev2, step,
+                            next_table, dims, stream);
 }
 
 extern "C" int lp_boundary_gradient_estimation(const lp_heads* model_out, const float* y, const float* noise,
                                                const uint8_t* mask, const lp_known* known, float* x_inout, float* out,
                                                float* d_out, const float* d_prev, const lp_gradient_estimation* step,
                                                const float* next_table, const lp_dims* dims, lp_stream_t stream) {
-  return boundary_ge_impl(model_out, y, noise, mask, known, x_inout, out, d_out, d_prev, step, next_table, dims,
+  return boundary_ge_impl(model_out, y, noise, mask, known, x_inout, out, -1, d_out, d_prev, step, next_table, dims,
                           stream);
+}
+
+extern "C" int lp_boundary_gradient_estimation_rows(const lp_heads* model_out, const float* y, const float* noise,
+                                                    const uint8_t* mask, const lp_known* known, float* x_inout,
+                                                    float* out, int64_t out_rows, float* d_out, const float* d_prev,
+                                                    const lp_gradient_estimation* step, const float* next_table,
+                                                    const lp_dims* dims, lp_stream_t stream) {
+  if (out_rows < 0) return LP_ERR_INVALID;
+  return boundary_ge_impl(model_out, y, noise, mask, known, x_inout, out, out_rows, d_out, d_prev, step, next_table,
+                          dims, stream);
 }
 
 extern "C" int lp_boundary_heun(const lp_heads* model_out, const float* y, const float* noise, const uint8_t* mask,
@@ -1372,14 +1428,14 @@ extern "C" int lp_epilogue_f32(const float* model_out, const float* y, const uin
                                const lp_dims* dims, lp_stream_t stream) {
   if (!out) return LP_ERR_INVALID;
   lp_heads h = {model_out, nullptr, LP_DTYPE_F32, 0, 0.f, 0.f};
-  return boundary_impl(&h, y, nullptr, mask, nullptr, nullptr, out, 0.f, nullptr, dims, stream);
+  return boundary_impl(&h, y, nullptr, mask, nullptr, nullptr, out, -1, 0.f, nullptr, dims, stream);
 }
 
 extern "C" int lp_epilogue_euler_f32(const float* model_out, const float* y, const uint8_t* mask, float* x_inout,
                                      float* out, float euler_coef, const lp_dims* dims, lp_stream_t stream) {
   if (!x_inout) return LP_ERR_INVALID;
   lp_heads h = {model_out, nullptr, LP_DTYPE_F32, 0, 0.f, 0.f};
-  return boundary_impl(&h, y, nullptr, mask, nullptr, x_inout, out, euler_coef, nullptr, dims, stream);
+  return boundary_impl(&h, y, nullptr, mask, nullptr, x_inout, out, -1, euler_coef, nullptr, dims, stream);
 }
 
 extern "C" int lp_step_boundary_f32(const float* model_out, const float* y, const float* noise, const uint8_t* mask,
@@ -1387,7 +1443,7 @@ extern "C" int lp_step_boundary_f32(const float* model_out, const float* y, cons
                                     const lp_dims* dims, lp_stream_t stream) {
   if (!noise || !x_inout || !next_table) return LP_ERR_INVALID;
   lp_heads h = {model_out, nullptr, LP_DTYPE_F32, 0, 0.f, 0.f};
-  return boundary_impl(&h, y, noise, mask, nullptr, x_inout, out, euler_coef, next_table, dims, stream);
+  return boundary_impl(&h, y, noise, mask, nullptr, x_inout, out, -1, euler_coef, next_table, dims, stream);
 }
 
 extern "C" int lp_epilogue_cfg_f32(const float* cond, const float* uncond, float cfg, const float* y,
@@ -1395,7 +1451,7 @@ extern "C" int lp_epilogue_cfg_f32(const float* cond, const float* uncond, float
                                    const lp_dims* dims, lp_stream_t stream) {
   if (!cond || !uncond || !out) return LP_ERR_INVALID;
   lp_heads h = {cond, uncond, LP_DTYPE_F32, 1, cfg, cfg};
-  return boundary_impl(&h, y, nullptr, mask, nullptr, x_inout, out, euler_coef, nullptr, dims, stream);
+  return boundary_impl(&h, y, nullptr, mask, nullptr, x_inout, out, -1, euler_coef, nullptr, dims, stream);
 }
 
 extern "C" int lp_advance_f32(float* x_model, const float* c_state, const uint8_t* mask, const float* table,

@@ -534,7 +534,7 @@ class LanPaint:
     def _launch_sequence(self, xm, y, nz, pm, dims, tab, t_model, sigma_dev, cbuf, out, active, plan, call_scaling,
                          model_options, seed, stopper, rng_state, euler_coef=None, skip_prologue=False,
                          next_table=None, current_times=None, ancestral=None, discard_heads=False, multistep=None,
-                         midpoint=None, deis=None, ge=None, heun=None):
+                         midpoint=None, deis=None, ge=None, heun=None, out_rows=None):
         """discard_heads: the caller owns the network's outputs and nothing reads them once the update kernel that
         consumes them has run (`heads_discardable`), so that kernel may drop them from the L2 unwritten
         (LP_HEADS_DEAD).  Only the fused loop's launches take it; the early-stop loop hands the heads to the stopper.
@@ -548,7 +548,9 @@ class LanPaint:
         lp_boundary_gradient_estimation, the update of a host-owned sample_gradient_estimation loop.
         heun: (lp_heun, x_base, out_prev): the boundary is lp_boundary_heun, the corrector of a host-owned sample_heun
         loop, with x_base (the state the step started from, updated in place) as its x, xm -- the state this call's
-        sub-steps ran on -- as its x2, and out_prev the step's first call's denoised latent."""
+        sub-steps ran on -- as its x2, and out_prev the step's first call's denoised latent.
+        out_rows: `out` holds only its first out_rows rows (the boundary's row-bounded form, lp_boundary_*_rows);
+        None: every row.  Not for multistep and heun, whose out a later launch reads whole."""
         lib = _native.load()
         dev = xm.device
         stream = _P(_stream_ptr(dev))
@@ -659,17 +661,20 @@ class LanPaint:
         else:
             mo, _ = self.unpack_model_output(out_heads)
             hd, keep = _heads(mo, None, xm, dead=discard_heads)
+        rows = () if out_rows is None else (out_rows,)   # the out_rows argument of the row-bounded forms
+        if (multistep is not None or heun is not None) and rows:
+            raise ValueError("the multistep and heun boundaries store every row of out")
         if ancestral is not None:
             # host-owned sample_euler_ancestral loop: (lp_ancestral, whether the sampler draws at this step).  Its
             # randn_like comes after the step's Langevin draws, so its position is taken here, not earlier
             step, draws = ancestral
             r = plan.rng_struct(1, rng_state) if draws else None
-            rc = lib.lp_boundary_ancestral(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
-                                           C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
-                                           _P(xm.data_ptr()), _P(_ptr(out)), C.byref(step),
-                                           C.byref(r) if r is not None else None,
-                                           _P(next_table.data_ptr()) if next_table is not None else None,
-                                           C.byref(dims), stream)
+            rc = (lib.lp_boundary_ancestral_rows if rows else lib.lp_boundary_ancestral)(
+                C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
+                C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
+                _P(xm.data_ptr()), _P(_ptr(out)), *rows, C.byref(step),
+                C.byref(r) if r is not None else None, _P(next_table.data_ptr()) if next_table is not None else None,
+                C.byref(dims), stream)
             _native.check(rc, "lp_boundary_ancestral")
             self.launches += 1
             return done
@@ -685,30 +690,30 @@ class LanPaint:
             return done
         if midpoint is not None:
             step, x_base, x_out = midpoint
-            rc = lib.lp_boundary_midpoint(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
-                                          C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
-                                          _P(xm.data_ptr()), _P(x_base.data_ptr()), _P(x_out.data_ptr()), _P(_ptr(out)),
-                                          C.byref(step), _P(next_table.data_ptr()) if next_table is not None else None,
-                                          C.byref(dims), stream)
+            rc = (lib.lp_boundary_midpoint_rows if rows else lib.lp_boundary_midpoint)(
+                C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
+                C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
+                _P(xm.data_ptr()), _P(x_base.data_ptr()), _P(x_out.data_ptr()), _P(_ptr(out)), *rows,
+                C.byref(step), _P(next_table.data_ptr()) if next_table is not None else None, C.byref(dims), stream)
             _native.check(rc, "lp_boundary_midpoint")
             self.launches += 1
             return done
         if deis is not None:
             step, d_out, p1, p2 = deis
-            rc = lib.lp_boundary_deis(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
-                                      C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
-                                      _P(xm.data_ptr()), _P(_ptr(out)), _P(_ptr(d_out)), _P(_ptr(p1)), _P(_ptr(p2)),
-                                      C.byref(step), _P(next_table.data_ptr()) if next_table is not None else None,
-                                      C.byref(dims), stream)
+            rc = (lib.lp_boundary_deis_rows if rows else lib.lp_boundary_deis)(
+                C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
+                C.byref(kn.struct) if kn is not None and kn.noise is not None else None,
+                _P(xm.data_ptr()), _P(_ptr(out)), *rows, _P(_ptr(d_out)), _P(_ptr(p1)), _P(_ptr(p2)),
+                C.byref(step), _P(next_table.data_ptr()) if next_table is not None else None, C.byref(dims), stream)
             _native.check(rc, "lp_boundary_deis")
             self.launches += 1
             return done
         if ge is not None:
             step, d_out, d_prev = ge
-            rc = lib.lp_boundary_gradient_estimation(
+            rc = (lib.lp_boundary_gradient_estimation_rows if rows else lib.lp_boundary_gradient_estimation)(
                 C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()), _P(pm.data.data_ptr()),
                 C.byref(kn.struct) if kn is not None and kn.noise is not None else None, _P(xm.data_ptr()),
-                _P(_ptr(out)), _P(_ptr(d_out)), _P(_ptr(d_prev)), C.byref(step),
+                _P(_ptr(out)), *rows, _P(_ptr(d_out)), _P(_ptr(d_prev)), C.byref(step),
                 _P(next_table.data_ptr()) if next_table is not None else None, C.byref(dims), stream)
             _native.check(rc, "lp_boundary_gradient_estimation")
             self.launches += 1
@@ -725,11 +730,12 @@ class LanPaint:
             return done
         fused_next = next_table is not None and euler_coef is not None
         if kn is not None and (kn.noise is not None or not fused_next):
-            rc = lib.lp_boundary_known(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()) if fused_next else None,
-                                       _P(pm.data.data_ptr()), C.byref(kn.struct),
-                                       _P(xm.data_ptr()) if euler_coef is not None else None, _P(_ptr(out)),
-                                       C.c_float(euler_coef or 0.0), _P(next_table.data_ptr()) if fused_next else None,
-                                       C.byref(dims), stream)
+            rc = (lib.lp_boundary_known_rows if rows else lib.lp_boundary_known)(
+                C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()) if fused_next else None, _P(pm.data.data_ptr()),
+                C.byref(kn.struct), _P(xm.data_ptr()) if euler_coef is not None else None, _P(_ptr(out)), *rows,
+                C.c_float(euler_coef or 0.0), _P(next_table.data_ptr()) if fused_next else None, C.byref(dims), stream)
+        elif rows:
+            raise ValueError("a row-bounded out needs the known-operand layout")
         else:
             rc = lib.lp_boundary(C.byref(hd), _P(y.data_ptr()), _P(nz.data_ptr()) if fused_next else None,
                                  _P(pm.data.data_ptr()), _P(xm.data_ptr()) if euler_coef is not None else None,

@@ -588,7 +588,9 @@ class GraphedJob:
         self._graphs = {}
         self._dims = None
         self.timing, self.last_events = False, None
+        self.first_step_end = None   # mode "eager": an event recorded after the first outer step
         self.outs = None     # per-outer-step denoised latents (mode "job" with a callback: callbacks run after the replay)
+        self._outs = {}      # observe setting -> its `outs`, kept as long as the graphs that write them
         self.launches = 0
         self.model_calls = 0
         self.captures = 0
@@ -601,16 +603,51 @@ class GraphedJob:
     @property
     def graph(self):
         """The whole-job graph (None until the first mode="job" run)."""
-        return self._graphs.get(("job", False))
+        return self._graphs.get(("job", False, "full"))
 
     def per_step_bytes(self) -> int:
         return len(self.sched.steps) * self.x.numel() * 4
 
     def denoised_buffer(self, i: int, want_out) -> torch.Tensor:
-        """Where outer step i writes its denoised latent (mode "job" with a callback: its own buffer)."""
+        """Where outer step i writes its denoised latent (mode "job" with a callback: its own buffer, see `_observed`)."""
         if want_out == "each":
             return self.outs[i]
         return self.out_pair[i % 2] if self.out_pair is not None else self.out
+
+    def _out_whole(self, i: int) -> bool:
+        """Whether outer step i stores its whole denoised latent whatever the callback reads: a later launch reads it
+        (the un-fused update, the multistep samplers' next step, heun's corrector), or its boundary,
+        lp_boundary_multistep, has no row-bounded form."""
+        if not self.fused_euler:
+            return True
+        if self.multistep is not None:
+            read = i + 1 < len(self.sched.steps) and self.multistep[i + 1][1]
+            return read or not isinstance(self.multistep[i][0], _native.Midpoint)
+        return self.sampler == "heun" and self.midpoint[i][2] is not None
+
+    def _observed(self, observe: str):
+        """`outs` of mode "job" with a callback: per outer step, the buffer its denoised latent goes to.  "full": every
+        step's whole latent.  "preview": before the last step, only row 0 -- all a latent preview decodes -- into a
+        [1, ...] buffer; "final": nothing.  The last step, and every step `_out_whole` names, keep the whole latent."""
+        if observe not in ("full", "preview", "final"):
+            raise ValueError(f"unknown observe setting {observe!r}")
+        outs = self._outs.get(observe)
+        if outs is None:
+            n = len(self.sched.steps)
+            outs = []
+            for i in range(n):
+                if observe == "full" or i + 1 == n or self._out_whole(i):
+                    outs.append(torch.empty_like(self.x))
+                elif observe == "preview":
+                    outs.append(torch.empty((1,) + self.shape[1:], dtype=torch.float32, device=self.device))
+                else:
+                    outs.append(None)
+            self._outs[observe] = outs
+        return outs
+
+    def _out_rows(self, out):
+        """The out_rows argument of a boundary that writes `out`: None (every row) unless `out` holds fewer rows."""
+        return out.shape[0] if out is not None and out.shape[0] < self.shape[0] else None
 
     # ---- the body ------------------------------------------------------------------------------
     def _init_state(self):
@@ -654,7 +691,8 @@ class GraphedJob:
                              ancestral=anc if self.fused_euler else None,
                              multistep=(ms[0], old) if (self.fused_euler and ms is not None and not euler_mp) else None,
                              midpoint=(ms[0], self.x, self.x) if (self.fused_euler and euler_mp) else None,
-                             deis=dz if self.fused_euler else None, ge=ge if self.fused_euler else None)
+                             deis=dz if self.fused_euler else None, ge=ge if self.fused_euler else None,
+                             out_rows=self._out_rows(out))
         if self.fused_euler:
             return
         if self.sampler == "res_multistep":     # sample_res_multistep's tensor ops, in its order
@@ -736,7 +774,7 @@ class GraphedJob:
                              self.rng_state.data_ptr(), discard_heads=dead,
                              skip_prologue=(fused and i > 0) or (i == 0 and self.first_replace_noop),
                              next_table=(self.mid_tables[k] if k is not None else after) if fused else None,
-                             midpoint=(pred, self.x, x_a) if fused else None)
+                             midpoint=(pred, self.x, x_a) if fused else None, out_rows=self._out_rows(out))
         sc = self.call_scalars[i]
         if not fused:   # the sampler's tensor ops, in its order
             d = (self.x - out) / sc[0]
@@ -841,9 +879,14 @@ class GraphedJob:
         self.mask.known = pack_known(self.mask, self._dims, self.y, self.noise, out=self.mask.known)
 
     def run(self, latent_image: torch.Tensor, noise: torch.Tensor, mask, x_out: Optional[torch.Tensor] = None,
-            x_init: Optional[torch.Tensor] = None, callback=None, mode: Optional[str] = None, warm: bool = True):
+            x_init: Optional[torch.Tensor] = None, callback=None, mode: Optional[str] = None, warm: bool = True,
+            observe: str = "full"):
         """callback(i, denoised, x, total_steps) is called on the host after outer step i has been ENQUEUED
-        (it sees device tensors in stream order; a callback that only counts steps never synchronises)."""
+        (it sees device tensors in stream order; a callback that only counts steps never synchronises).
+
+        observe (mode "job" with a callback): what of each step's denoised latent the callback is handed, see
+        `_observed` -- "full", "preview" (before the last step, the [1, ...] latent of the first request) or "final"
+        (before the last step, an empty [0, ...] tensor).  The last step's is always whole."""
         import numpy as np
         eng = self.engine
         if self.external_init != (x_init is not None):
@@ -863,16 +906,19 @@ class GraphedJob:
             n_steps = len(self.sched.steps)
             want_out = callback is not None
             if mode == "job":
-                if want_out and self.outs is None:
-                    self.outs = [torch.empty_like(self.x) for _ in range(n_steps)]
+                if want_out:
+                    self.outs = self._observed(observe)
+                else:
+                    observe = "full"
                 each = "each" if want_out else False
-                graph, stats = self._graph_for(("job", each), lambda p: self._body(p, each), warm)
+                graph, stats = self._graph_for(("job", each, observe), lambda p: self._body(p, each), warm)
                 graph.replay()
                 eng.launches += stats[0]
                 eng.model_calls += stats[1]
                 if callback is not None:
                     for i in range(n_steps):
-                        callback(i, self.outs[i], self.x, n_steps)
+                        out = self.outs[i]
+                        callback(i, out if out is not None else self.outs[-1][:0], self.x, n_steps)
             elif mode == "steps":
                 if not self.external_init:
                     self._init_state()
@@ -891,6 +937,9 @@ class GraphedJob:
                     self._step(i, rel, want_out)
                     if callback is not None:
                         callback(i, self.denoised_buffer(i, want_out), self.x, n_steps)
+                    if i == 0:   # the first outer step also pays the process's first launches (CUDA's lazy loading)
+                        self.first_step_end = torch.cuda.Event(enable_timing=True)
+                        self.first_step_end.record()
             else:
                 raise ValueError(f"unknown mode {mode!r}")
             if self.timing:

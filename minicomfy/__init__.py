@@ -682,14 +682,35 @@ def common_ksampler(model, seed, steps, cfg, sampler_name, scheduler, positive, 
 
 
 PROGRESS = {"calls": 0, "last": None}
+PREVIEW = {"previewer": None}     # what get_previewer returns (ComfyUI: per the --preview-method setting)
+
+
+class Latent2RGBPreviewer:
+    """ComfyUI's latent-to-RGB previewer, as far as a caller can observe it: it decodes the first request's latent,
+    x0[:1], here kept as a device copy per call."""
+
+    def __init__(self):
+        self.seen = []
+
+    def decode_latent_to_preview_image(self, preview_format, x0):
+        self.seen.append(x0[:1].clone())
+        return None
+
+
+def get_previewer(device=None, latent_format=None):
+    return PREVIEW["previewer"]
 
 
 def prepare_callback(model, steps, x0_output_dict=None):
-    """ComfyUI's latent_preview.prepare_callback with no previewer configured: keeps the latest x0 for the
-    custom-sampler nodes and advances the progress bar; never reads device memory."""
+    """ComfyUI's latent_preview.prepare_callback: keeps the latest x0 for the custom-sampler nodes, hands it to the
+    previewer when one is configured (none by default) and advances the progress bar."""
+    previewer = get_previewer()
+
     def callback(step, x0, x, total_steps):
         if x0_output_dict is not None:
             x0_output_dict["x0"] = x0
+        if previewer:
+            previewer.decode_latent_to_preview_image("JPEG", x0)
         PROGRESS["calls"] += 1
         PROGRESS["last"] = (step + 1, total_steps)
     return callback
@@ -736,7 +757,8 @@ def install(version: str = "0.6.0") -> None:
                        fix_empty_latent_channels=fix_empty_latent_channels)
     comfy.model_management = mod("comfy.model_management", intermediate_device=intermediate_device)
     mod("nodes", common_ksampler=common_ksampler)
-    mod("latent_preview", prepare_callback=prepare_callback)
+    mod("latent_preview", prepare_callback=prepare_callback, get_previewer=get_previewer,
+        Latent2RGBPreviewer=Latent2RGBPreviewer)
     mod("comfyui_version", __version__=version)
 
 
