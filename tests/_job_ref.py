@@ -17,6 +17,7 @@ with; in fp32 it reproduces the reference's node layer on the node fixtures' tap
 """
 from __future__ import annotations
 
+import functools
 import math
 from unittest import mock
 
@@ -146,4 +147,8 @@ def job(sampler, model, y, noise, denoise_mask, sigmas, hp: O.Hyper, draw=cuda_d
 
 
 SAMPLERS = {"euler": _plain(minicomfy.sample_euler), "heun": _plain(minicomfy.sample_heun),
-            "euler_ancestral": _euler_ancestral}
+            "euler_ancestral": _euler_ancestral, "dpmpp_2m": _plain(minicomfy.sample_dpmpp_2m),
+            "dpm_2": _plain(minicomfy.sample_dpm_2), "deis": _plain(minicomfy.sample_deis),
+            # its noise sampler is seeded from extra_args, and its draws are multiplied by sigma_up = 0 (eta = 0)
+            "res_multistep": _plain(functools.partial(minicomfy.sample_res_multistep, extra_args={"seed": 0})),
+            "gradient_estimation": _plain(minicomfy.sample_gradient_estimation)}
